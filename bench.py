@@ -2,7 +2,7 @@
 """bench.py — leapfrog-steps/s of the many-chain NUTS hot path (BASELINE.json metric).
 
 Default workload at N=1 (BASELINE.json configs[1], "C2"): 1000-dim standard MvNormal, 65 536 chains, diagonal M⁻¹,
-FP64, 1×B200.  Setup (untimed): random start, initial step-size search, one dual-averaging stage so that ϵ is
+FP64, 1×H100.  Setup (untimed): random start, initial step-size search, one dual-averaging stage so that ϵ is
 adapted per chain.  A timed "step" = one pass of the hot path over the batch: `draws_per_step` NUTS transitions for
 every chain (dhmc_mcmc_dev, state and outputs in HBM).  `value` = Σ tree_statistics.steps ÷ device time (CUDA events
 on the library's stream, max over ranks); `e2e` repeats the same step through the host-buffer C ABI call
@@ -39,9 +39,10 @@ import __graft_entry__ as entry  # noqa: E402
 
 METRIC = "leapfrog_steps_per_sec"
 UNIT = "leapfrog-steps/s"
-# FP64 tensor-core (DMMA m8n8k4) rate measured on this pool's B200 by benchmarks/c4_probes.cu
-# (profiles/r02_c4_probes.txt): 64 FMA/clk/SM — the same as the DFMA pipe; x 148 SMs x SM clock x 2 flop
-DMMA_FMA_PER_CLK_SM = 64.0
+# FP64 tensor-core (DMMA) rate of the H100 SXM data sheet: 67 TFLOP/s = 128 FMA/clk/SM x 132 SMs x 1980 MHz x 2 flop
+# (a data-sheet figure, not a measurement: benchmarks/c4_probes.cu measures the rate); the roofline scales it by the
+# device's SM count and clock
+DMMA_FMA_PER_CLK_SM = 128.0
 
 
 def peaks():
@@ -49,10 +50,10 @@ def peaks():
     if os.path.exists(p):
         try:
             d = json.load(open(p))
-            return float(d["hbm_gbs"]), float(d.get("sm_max_mhz", 1965.0)), "measured"
+            return float(d["hbm_gbs"]), float(d.get("sm_max_mhz", 1980.0)), "measured"
         except Exception:
             pass
-    return 6650.0, 1965.0, "fallback"
+    return 3350.0, 1980.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3, 1980 MHz max SM clock)"
 
 
 def usable_cores():
@@ -88,10 +89,10 @@ def cpu_model():
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks/throttle reasons during the timed region (read-only queries)."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
-         "clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.sw_power_cap,power.limit")
 
     def __init__(self, index):
         self.index, self.rows, self.proc = index, [], None
@@ -112,25 +113,25 @@ class ClockSampler:
 
     def stop(self):
         if not self.proc:
-            return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
+            return {"sm_mhz": None, "sm_max_mhz": None, "power_limit_w": None, "reasons": ["nvidia-smi unavailable"]}
         time.sleep(0.25)
         self.proc.terminate()
         try:
             self.proc.wait(timeout=2)
         except Exception:
             pass
-        sm, mx, reasons = [], [], set()
+        sm, mx, plim, reasons = [], [], [], set()
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         for r in self.rows:
             try:
-                sm.append(float(r[0])); mx.append(float(r[1]))
+                sm.append(float(r[0])); mx.append(float(r[1])); plim.append(float(r[7]))
                 for n, v in zip(names, r[3:7]):
                     if v.lower().startswith("active"):
                         reasons.add(n)
             except Exception:
                 continue
         return {"sm_mhz": float(np.median(sm)) if sm else None,
-                "sm_max_mhz": float(np.max(mx)) if mx else None,
+                "sm_max_mhz": float(np.max(mx)) if mx else None, "power_limit_w": float(np.max(plim)) if plim else None,
                 "reasons": sorted(reasons), "samples": len(sm)}
 
 
@@ -288,11 +289,12 @@ def user_model_leg(pkg, wl, K, D, n, args, local_rank, chain_offset, draws, stat
         return {"error": "%s: %s" % (type(e).__name__, str(e)[:300])}
 
 
-def c4_probe_leg(pkg, torch, dev, local_rank, sm_max_mhz, chains=4736, warm=(20, 40, 20), draws=4):
+def c4_probe_leg(pkg, torch, dev, local_rank, sm_max_mhz, sm_count, warm=(20, 40, 20), draws=4):
     """The tensor-core kernel of BASELINE.json configs[3] (logistic N=10 000, p=256, per-chain dense metric) inside the default
-    run, at a REDUCED chain count (4 736 = 4 waves of 148 SMs x 8 chains per CTA instead of 32 768, so that the default bench
+    run, at a REDUCED chain count (4 waves of the device's SMs x 8 chains per CTA instead of 32 768, so that the default bench
     stays short): search + TuningNUTS(20) + TuningNUTS(40, Symmetric) + TuningNUTS(20), then `draws` timed transitions with the
-    adapted dense metric.  The full-size line is `bench.py --config C4` (profiles/r02_bench_c4.json).  Never fails the bench."""
+    adapted dense metric.  The full-size line is `bench.py --config C4`.  Never fails the bench."""
+    chains = 4 * sm_count * 8
     try:
         N, p = 10000, 256
         ℓ, _ = pkg.LogisticRegression.synthetic(N=N, p=p, seed=7)
@@ -319,7 +321,7 @@ def c4_probe_leg(pkg, torch, dev, local_rank, sm_max_mhz, chains=4736, warm=(20,
             summary = eng.tree_summary_dev(stats.data_ptr(), 1, ebfmi=False)
         finally:
             eng.close()
-        peak_tf = DMMA_FMA_PER_CLK_SM * 2 * 148 * sm_max_mhz * 1e6 / 1e12
+        peak_tf = DMMA_FMA_PER_CLK_SM * 2 * sm_count * sm_max_mhz * 1e6 / 1e12
         rate, wrate = steps / (ms * 1e-3), w_steps / (w_ms * 1e-3)
         return {"workload": "C4 kernel probe: logistic regression N=%d p=%d, %d chains (full size: 32768), per-chain dense metric adapted by "
                             "search + TuningNUTS(%d) + TuningNUTS(%d, Symmetric) + TuningNUTS(%d); likelihood and M^-1 p on DMMA.8x8x4"
@@ -328,16 +330,16 @@ def c4_probe_leg(pkg, torch, dev, local_rank, sm_max_mhz, chains=4736, warm=(20,
                 "warmup_value": wrate, "warmup_tflops_fp64": wrate * flops / 1e12, "dmma_peak_tflops": peak_tf,
                 "leapfrogs_per_transition": steps / (draws * chains), "a_mean": summary["a_mean"],
                 "depth_counts": summary["depth_counts"], "seconds": time.perf_counter() - t0,
-                "what": "device-timed like `value`, run after the timed region of the default workload; 4736 of the 32768 C4 chains, so "
-                        "tail effects of the last wave weigh more than at full size"}
+                "what": "device-timed like `value`, run after the timed region of the default workload; %d of the 32768 C4 chains, so "
+                        "tail effects of the last wave weigh more than at full size" % chains}
     except Exception as e:
         return {"error": "%s: %s" % (type(e).__name__, str(e)[:300])}
 
 
 def c3_probe_leg(pkg, torch, dev, local_rank, chains=262144, draws=10):
     """BASELINE.json configs[2] at FULL size inside the default run: Neal's funnel D=10, 262 144 chains, the default warm-up
-    (900 transitions, ragged tree depths), then `draws` timed transitions.  Same code as `bench.py --config C3`
-    (profiles/r02_bench_c3.json).  Never fails the bench."""
+    (900 transitions, ragged tree depths), then `draws` timed transitions.  Same code as `bench.py --config C3`.
+    Never fails the bench."""
     try:
         t0 = time.perf_counter()
         eng = pkg.Engine(pkg.Funnel(10), chains=chains, seed=2026, device=local_rank)
@@ -370,6 +372,24 @@ def c3_probe_leg(pkg, torch, dev, local_rank, chains=262144, draws=10):
         return {"error": "%s: %s" % (type(e).__name__, str(e)[:300])}
 
 
+def dump_outputs(out_dir, pkg, torch, draws, stats, logd, limit=60_000_000):
+    """What the timed path returned in its last step, as out_dir/<name>.npy: the draws [chains, draws_per_step, dim], the log
+    densities and every field of the tree statistics [chains, draws_per_step], float64.  Above `limit` bytes in all, a fixed
+    seeded sample of the chains is written (ascending; its indices as chains.npy)."""
+    K, n, D = draws.shape
+    fields = [f for f in pkg._lib.tree_stats_dtype.names if f != "pad"]
+    m = min(K, limit // (8 * n * (D + 1 + len(fields)) + 8))
+    idx = np.arange(K) if m == K else np.sort(np.random.default_rng(0).choice(K, size=m, replace=False))
+    sel = torch.from_numpy(idx).to(draws.device)
+    st = stats.index_select(0, sel).cpu().numpy().view(pkg._lib.tree_stats_dtype).reshape(m, n)
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "chains.npy"), idx.astype(np.float64))
+    np.save(os.path.join(out_dir, "posterior_matrix.npy"), draws.index_select(0, sel).cpu().numpy())
+    np.save(os.path.join(out_dir, "logdensities.npy"), logd.index_select(0, sel).cpu().numpy())
+    for f in fields:
+        np.save(os.path.join(out_dir, f"tree_statistics_{f}.npy"), st[f].astype(np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -388,6 +408,8 @@ def main():
     ap.add_argument("--ref-seconds", type=float, default=1.2)
     ap.add_argument("--cpu-baseline-seconds", type=float, default=4.0)
     ap.add_argument("--skip-e2e", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step (draws, log densities, tree statistics) as DIR/<name>.npy")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -413,6 +435,7 @@ def main():
     wl = make_workload(pkg, args.config, args)
     D, n = wl["dim"], wl["draws"]
     dev = torch.device("cuda", local_rank)
+    props = torch.cuda.get_device_properties(local_rank)
 
     def barrier():
         if world > 1:
@@ -459,6 +482,8 @@ def main():
     wall = time.perf_counter() - t0
     clocks = sampler.stop()
     launches = eng.kernel_launches() - launches0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, pkg, torch, draws, stats, logd)
     summary = eng.tree_summary_dev(stats.data_ptr(), n, ebfmi=False) if rank == 0 else None
     q_typical = None if args.skip_e2e else eng.get_state(("q",))["q"]   # posterior draws: the e2e steps start from them
 
@@ -518,7 +543,7 @@ def main():
     # own kernel at a reduced chain count, configs[2] at full size.  DHMC_BENCH_NO_PROBES=1 skips them.
     c4_leg = c3_leg = None
     if world == 1 and args.config == "C2" and not args.chains and not args.dim and not os.environ.get("DHMC_BENCH_NO_PROBES"):
-        c4_leg = c4_probe_leg(pkg, torch, dev, local_rank, peaks()[1])
+        c4_leg = c4_probe_leg(pkg, torch, dev, local_rank, peaks()[1], props.multi_processor_count)
         c3_leg = c3_probe_leg(pkg, torch, dev, local_rank)
 
     # ---------------- multi-GPU: one NCCL all-gather of the draws (library communicator), after timing ----------------
@@ -553,22 +578,12 @@ def main():
         kernel = ("k_nuts<logistic, 8 chains per CTA, tensor-core likelihood + mat-vec>" if packed
                   else "k_nuts (whole NUTS transition, chain state resident on chip)")
         if wl["flops_per_lf"]:
-            peak_tf = DMMA_FMA_PER_CLK_SM * 2 * 148 * sm_max_mhz * 1e6 / 1e12
+            peak_tf = DMMA_FMA_PER_CLK_SM * 2 * props.multi_processor_count * sm_max_mhz * 1e6 / 1e12
             ach = steps_per_launch * wl["flops_per_lf"] / (ms_per_launch * 1e-3) / 1e12
-            traffic, traffic_src = None, None
-            try:   # the ncu capture ran a smaller batch; the traffic is the per-chain metric stream, i.e. proportional to the steps
-                tr = json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json")))["c4"]
-                per_ms = (tr["dram_bytes_read"] + tr["dram_bytes_write"]) / tr["duration_ms"]
-                traffic = per_ms * ms_per_launch
-                traffic_src = ("scaled by launch duration from the committed ncu --set full capture at %d chains (profiles/r02_traffic.json: "
-                               "%.0f GB in %.0f ms = %.2f TB/s, the per-chain dense metrics), not measured in this run"
-                               % (tr["chains"], (tr["dram_bytes_read"] + tr["dram_bytes_write"]) / 1e9, tr["duration_ms"], per_ms / 1e9))
-            except Exception:
-                pass
             roof = {"bound": "tensor", "kernel": kernel, "achieved": ach, "peak": peak_tf, "unit": "TFLOP/s",
-                    "frac": ach / peak_tf, "traffic": traffic, "traffic_source": traffic_src,
-                    "peak_kind": "FP64 DMMA rate measured by benchmarks/c4_probes.cu (64 FMA/clk/SM = the DFMA rate) x 148 SMs x "
-                                 "%.0f MHz; MEASURED_PEAKS.json holds no FP64 figure" % sm_max_mhz,
+                    "frac": ach / peak_tf, "traffic": None, "traffic_source": "not measured",
+                    "peak_kind": "FP64 DMMA rate of the H100 SXM data sheet (%.0f FMA/clk/SM) x %d SMs x %.0f MHz; MEASURED_PEAKS.json "
+                                 "holds no FP64 figure" % (DMMA_FMA_PER_CLK_SM, props.multi_processor_count, sm_max_mhz),
                     "algorithmic_flops_per_launch": steps_per_launch * wl["flops_per_lf"],
                     "flops_per_leapfrog": wl["flops_per_lf"]}
             # the per-chain dense metric is a GEMV stream from HBM: 2 mat-vecs per leapfrog, each over the chain's padded
@@ -583,19 +598,10 @@ def main():
                                                   "n-dimension carries one vector); DHMC_METRIC_SYMMETRIC_POOLED turns it into a GEMM"}
         else:
             ach = steps_per_launch * wl["bytes_per_lf"] / (ms_per_launch * 1e-3) / 1e9
-            traffic, traffic_src = None, None
-            try:   # DRAM bytes per launch from the committed ncu --set full capture of this same command
-                tr = json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json")))["k_nuts"]
-                if args.config == "C2" and (tr["dim"], tr["chains"], tr["draws_per_step"]) == (D, K, n):
-                    traffic = tr["dram_bytes_read"] + tr["dram_bytes_write"]
-                    traffic_src = "committed ncu --set full capture of this same command (profiles/r02_traffic.json), not measured in this run"
-            except Exception:
-                pass
             roof = {"bound": "hbm", "kernel": kernel, "achieved": ach, "peak": hbm_peak, "unit": "GB/s",
-                    "frac": ach / hbm_peak, "peak_kind": peak_kind, "traffic": traffic, "traffic_source": traffic_src,
+                    "frac": ach / hbm_peak, "peak_kind": peak_kind, "traffic": None, "traffic_source": "not measured",
                     "achieved_is": "HBM-EQUIVALENT: leapfrog steps per launch x %d B (algorithmic bytes, SURVEY 8d) / launch time; the "
                                    "kernel keeps q, p, grad on chip across the tree, so this is not DRAM bandwidth" % wl["bytes_per_lf"],
-                    "dram_frac": (traffic / (ms_per_launch * 1e-3) / 1e9 / hbm_peak) if traffic else None,
                     "algorithmic_bytes_per_launch": steps_per_launch * wl["bytes_per_lf"]}
         line = {
             "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps,
@@ -604,7 +610,7 @@ def main():
             "config": {"workload": f"{args.config}: {wl['label']}; {K} chains per GPU, NUTS (max_depth 10), FP64",
                        "dim": D, "chains_per_gpu": K, "draws_per_step": n, "threads_per_chain": T,
                        "elems_per_thread": EPL, "parallelism": f"chains sharded x{world}, no data-path collective",
-                       "l2": "state + outputs per step = %.2f GB > 126 MB L2" % ((3 + n) * K * D * 8 / 1e9),
+                       "l2": "state + outputs per step = %.2f GB, L2 = %.0f MB" % ((3 + n) * K * D * 8 / 1e9, props.L2_cache_size / 1e6),
                        "setup": wl["warm"], "setup_seconds": setup_s,
                        "warmup_leapfrog_steps_per_sec": (sm[9].item() / (mx[8].item() * 1e-3)) if mx[8].item() > 0 else None,
                        "mean_eps": float(np.mean(eps)), "leapfrogs_per_transition": tot_steps / (args.steps * n * K),
@@ -612,15 +618,11 @@ def main():
             "draws_per_sec": world * K * n * args.steps / (dev_ms_max * 1e-3),
             "wall_ms_per_step": 1e3 * wall_max / args.steps,
             "gpu_launches": int(sm[3].item()),
+            "gpu": props.name,
             "clocks": clocks,
             "roofline": roof,
             "tree_summary": {k: summary[k] for k in ("a_mean", "termination_counts", "depth_counts")} if summary else None,
         }
-        try:
-            rc = json.load(open(os.path.join(ROOT, "profiles", "r02_roofline_compute.json")))[args.config]
-            line["roofline_compute"] = rc
-        except Exception:
-            pass
         if lf_ms:
             line["roofline_leapfrog_stream"] = {"bound": "hbm", "kernel": "k_leapfrog (one leapfrog step per launch, HBM streaming)",
                                                 "achieved": lf_bytes / (lf_ms * 1e-3) / 1e9, "peak": hbm_peak, "unit": "GB/s",

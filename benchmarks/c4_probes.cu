@@ -1,6 +1,6 @@
 // c4_probes.cu — round-2 hardware probes behind the C4 (logistic regression) kernel design.
 //
-//   1. FP64 tensor-core rate and latency on sm_100a for mma.sync .f64 shapes m8n8k4 / m16n8k4 /
+//   1. FP64 tensor-core rate and latency on sm_90a for mma.sync .f64 shapes m8n8k4 / m16n8k4 /
 //      m16n8k8 / m16n8k16, next to the plain DFMA rate (is DMMA worth it, which shape, how many
 //      independent accumulator chains per warp hide the latency);
 //   2. the same m8n8k4 stream with its A fragment fetched from shared memory per instruction
@@ -8,14 +8,16 @@
 //   3. L2 → SM delivery when every SM sweeps the same 20 MB design matrix with cp.async.bulk
 //      (mbarrier complete_tx ring), all SMs in step vs. skewed starts vs. cluster-2 multicast.
 //
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o c4_probes c4_probes.cu
-// Run (B200): ./c4_probes
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o c4_probes c4_probes.cu
+// Run: ./c4_probes (one CTA per SM of device 0)
 #include <cuda_runtime.h>
 
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
 #include <vector>
+
+static int g_sms = 0;   // SMs of device 0: one CTA each
 
 #define CK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { std::printf("CUDA error %s at %s:%d\n", cudaGetErrorString(e_), __FILE__, __LINE__); std::exit(1); } } while (0)
 
@@ -72,15 +74,15 @@ __global__ void __launch_bounds__(1024, 1) k_rate(double* sink, long long* cycle
 template <int SHAPE, int CH>
 static void rate(const char* name, int warps, double* sink, long long* dcyc) {
   const int iters = 4096;
-  k_rate<SHAPE, CH><<<148, 32 * warps>>>(sink, dcyc, 64);
+  k_rate<SHAPE, CH><<<g_sms, 32 * warps>>>(sink, dcyc, 64);
   CK(cudaDeviceSynchronize());
-  k_rate<SHAPE, CH><<<148, 32 * warps>>>(sink, dcyc, iters);
+  k_rate<SHAPE, CH><<<g_sms, 32 * warps>>>(sink, dcyc, iters);
   CK(cudaDeviceSynchronize());
-  std::vector<long long> cyc(148);
-  CK(cudaMemcpy(cyc.data(), dcyc, 148 * sizeof(long long), cudaMemcpyDeviceToHost));
+  std::vector<long long> cyc(g_sms);
+  CK(cudaMemcpy(cyc.data(), dcyc, g_sms * sizeof(long long), cudaMemcpyDeviceToHost));
   double mean = 0;
   for (auto v : cyc) mean += (double)v;
-  mean /= 148;
+  mean /= g_sms;
   const double per_instr_warp = mean / ((double)iters * CH);                 // cycles between a warp's issues
   const double per_smsp = mean / ((double)iters * CH * ((warps + 3) / 4));   // cycles per instruction per SMSP
   const double fma_per_clk_sm = (double)Mma<SHAPE>::FMAS * iters * CH * warps / mean;
@@ -124,15 +126,15 @@ static void rate_lds(int warps, double* sink, long long* dcyc) {
   const int iters = 4096;
   const size_t smem = 64 * 260 * sizeof(double);
   CK(cudaFuncSetAttribute(k_rate_lds<CH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k_rate_lds<CH><<<148, 32 * warps, smem>>>(sink, dcyc, 64);
+  k_rate_lds<CH><<<g_sms, 32 * warps, smem>>>(sink, dcyc, 64);
   CK(cudaDeviceSynchronize());
-  k_rate_lds<CH><<<148, 32 * warps, smem>>>(sink, dcyc, iters);
+  k_rate_lds<CH><<<g_sms, 32 * warps, smem>>>(sink, dcyc, iters);
   CK(cudaDeviceSynchronize());
-  std::vector<long long> cyc(148);
-  CK(cudaMemcpy(cyc.data(), dcyc, 148 * sizeof(long long), cudaMemcpyDeviceToHost));
+  std::vector<long long> cyc(g_sms);
+  CK(cudaMemcpy(cyc.data(), dcyc, g_sms * sizeof(long long), cudaMemcpyDeviceToHost));
   double mean = 0;
   for (auto v : cyc) mean += (double)v;
-  mean /= 148;
+  mean /= g_sms;
   std::printf("rate m8n8k4+LDS.64 warps/SM %2d chains/warp %d : %6.2f clk/instr/SMSP  %7.1f FMA/clk/SM\n", warps, CH,
               mean / ((double)iters * CH * ((warps + 3) / 4)), 256.0 * iters * CH * warps / mean);
 }
@@ -272,23 +274,24 @@ static void sweep(const char* buf, size_t bytes, int sweeps, int skew, bool mc, 
     CK(cudaEventRecord(e0));
     if (mc) {
       CK(cudaFuncSetAttribute(k_sweep_mc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      k_sweep_mc<<<148, 256, smem>>>(buf, bytes, sweeps, skew, sink, dcyc);
+      k_sweep_mc<<<g_sms, 256, smem>>>(buf, bytes, sweeps, skew, sink, dcyc);
     } else {
       CK(cudaFuncSetAttribute(k_sweep, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      k_sweep<<<148, 256, smem>>>(buf, bytes, sweeps, skew, sink, dcyc);
+      k_sweep<<<g_sms, 256, smem>>>(buf, bytes, sweeps, skew, sink, dcyc);
     }
     CK(cudaEventRecord(e1));
     CK(cudaDeviceSynchronize());
     CK(cudaEventElapsedTime(&ms, e0, e1));
   }
-  const double tb = 148.0 * (double)bytes * sweeps / (ms * 1e-3) / 1e12;
+  const double tb = (double)g_sms * (double)bytes * sweeps / (ms * 1e-3) / 1e12;
   std::printf("sweep %-9s buf %5.1f MB x%d skew %4d : %8.3f ms  %6.2f TB/s delivered to the SMs (%5.1f GB/s per SM)\n",
-              mc ? "cluster2" : "unicast", bytes / 1e6, sweeps, skew, ms, tb, tb * 1e3 / 148);
+              mc ? "cluster2" : "unicast", bytes / 1e6, sweeps, skew, ms, tb, tb * 1e3 / g_sms);
 }
 
 int main() {
   double* sink; long long* dcyc;
-  CK(cudaMalloc(&sink, 8)); CK(cudaMalloc(&dcyc, 148 * sizeof(long long)));
+  CK(cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, 0));
+  CK(cudaMalloc(&sink, 8)); CK(cudaMalloc(&dcyc, g_sms * sizeof(long long)));
   int clk = 0;
   CK(cudaDeviceGetAttribute(&clk, cudaDevAttrClockRate, 0));
   std::printf("SM clock (max) %d kHz\n", clk);
@@ -304,7 +307,7 @@ int main() {
   rate<3, 1>("m16n8k16", 1, sink, dcyc); rate<3, 4>("m16n8k16", 4, sink, dcyc); rate<3, 2>("m16n8k16", 16, sink, dcyc);
   std::printf("--- m8n8k4 with the A fragment from shared memory\n");
   rate_lds<1>(16, sink, dcyc); rate_lds<2>(16, sink, dcyc); rate_lds<4>(16, sink, dcyc); rate_lds<4>(8, sink, dcyc);
-  std::printf("--- L2 -> SM sweeps (cp.async.bulk, 4 x 32 KB ring per SM, 148 CTAs)\n");
+  std::printf("--- L2 -> SM sweeps (cp.async.bulk, 4 x 32 KB ring per SM, %d CTAs)\n", g_sms);
   const size_t bytes = (size_t)20480000 / kTileBytes * kTileBytes;     // X: 10 000 x 256 doubles
   char* buf;
   CK(cudaMalloc(&buf, 2 * bytes));

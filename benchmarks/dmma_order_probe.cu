@@ -1,12 +1,12 @@
-// dmma_order_probe.cu — which summation order does mma.sync.m8n8k4.f64 use on sm_100a?
+// dmma_order_probe.cu — which summation order does mma.sync.m8n8k4.f64 use on sm_90a?
 //
 // Round-2 preparation (DESIGN.md §7, item (i)): the cooperative logistic likelihood is a
 // [rows × p]·[p × 8 chains] product, the shape of the FP64 tensor-core MMA.  To keep the oracle
 // bit-exact it has to restate the instruction's accumulation order, so this probe compares the
 // instruction against candidate orders on adversarial random inputs and reports the match counts.
 //
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O2 -fmad=false -o dmma_order_probe dmma_order_probe.cu
-// Run (B200): ./dmma_order_probe [trials]
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O2 -fmad=false -o dmma_order_probe dmma_order_probe.cu
+// Run: ./dmma_order_probe [trials]
 #include <cuda_runtime.h>
 
 #include <cmath>

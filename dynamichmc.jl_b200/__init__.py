@@ -1,6 +1,6 @@
-"""dynamichmc.jl_b200 — B200-native many-chain NUTS engine behind the
+"""dynamichmc.jl_b200 — H100-native many-chain NUTS engine behind the
 DynamicHMC.jl sampler API.  The numeric path is libdhmc_b200.so (hand-written
-sm_100a CUDA, csrc/); this package is the thin host mirror of the reference's
+sm_90a CUDA, csrc/); this package is the thin host mirror of the reference's
 interface over its C ABI.  There is no CPU fallback."""
 from . import _lib, diagnostics, parallel
 from .api import (ArgumentError, DiagNormal, Diagonal, DualAveraging, DynamicHMCError, Engine,

@@ -60,7 +60,7 @@ def lib(path=None):
         if not os.path.exists(path):
             raise MissingExtension(
                 f"{path} is missing: build it with `python -c 'import __graft_entry__ as g; "
-                "g.build()'` (nvcc, sm_100a).  dynamichmc.jl_b200 has no CPU fallback.")
+                "g.build()'` (nvcc, sm_90a).  dynamichmc.jl_b200 has no CPU fallback.")
         so = C.CDLL(path)
         so.dhmc_last_error.restype = C.c_char_p
         so.dhmc_last_error.argtypes = [C.c_void_p]

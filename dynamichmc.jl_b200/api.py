@@ -147,7 +147,7 @@ class LogisticRegression(DeviceLogDensity):
 # ------------------------------------------------------------------ user models
 # The reference accepts ANY LogDensityProblems object; its only use of it is logdensity_and_gradient at hamiltonian.jl:204.
 # On the device the counterpart is a header of scalar formulas (include/dhmc_models.h, "the model header contract";
-# examples in include/models/) that is compiled — nvcc, sm_100a, same flags as the shipped families — into its own copy of
+# examples in include/models/) that is compiled — nvcc, sm_90a, same flags as the shipped families — into its own copy of
 # the library, where it is family DHMC_FAMILY_USER.
 _CSRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), "csrc")
 

@@ -1,4 +1,4 @@
-// device_backend.cuh — sm_100a vector backend of the NUTS state machine.
+// device_backend.cuh — sm_90a vector backend of the NUTS state machine.
 //
 // One chain = one chain group of T = 32·W threads (= one CTA; packed chain groups of the
 // logistic family put 8 groups in a CTA, see coop_core).  Element i of
@@ -281,10 +281,9 @@ __device__ __noinline__ bool coop_core(double* sll_out, bool active, int tid, in
 
 // ---- the likelihood round on the FP64 tensor cores, fed by TMA bulk copies (default for packed groups) ----
 // mma.sync.m8n8k4.f64 (SASS DMMA.8x8x4) computes fma(a3,b3, fma(a2,b2, fma(a1,b1, fma(a0,b0, c))))
-// (measured: profiles/r01_dmma_order_probe.txt), i.e. the model's own sequential order, so the results
-// are those of coop_core bit for bit.  Measured on the B200 (profiles/r02_c4_probes.txt): one DMMA per
-// 16 clk per SM sub-partition = 64 FMA/clk/SM (the DFMA peak) with 1/8 of the instructions, latency
-// 26 clk, saturated by two independent accumulator chains per sub-partition.
+// (benchmarks/dmma_order_probe.cu; test_logistic_mma_likelihood_equals_fma_loops holds the kernels to it),
+// i.e. the model's own sequential order, so the results are those of coop_core bit for bit.  On the H100
+// the DMMA pipe has twice the DFMA rate (data sheet) with 1/8 of the instructions.
 //
 // One pass over the design matrix per gradient.  X is kept in HBM/L2 as zero-padded row blocks
 // [32 rows][XS] (XS ≡ 4 mod 16 doubles: every fragment load below is bank-conflict free); one elected

@@ -1,5 +1,5 @@
-// dhmc_b200.cu — sm_100a kernels and the C ABI (include/dhmc.h) of the
-// many-chain NUTS engine.  Build: see csrc/Makefile (nvcc -fmad=false, sm_100a).
+// dhmc_b200.cu — sm_90a kernels and the C ABI (include/dhmc.h) of the
+// many-chain NUTS engine.  Build: see csrc/Makefile (nvcc -fmad=false, sm_90a).
 //
 // Kernels (one chain group of T threads = one CTA; persistent, chains pulled
 // from an atomic queue so that ragged tree depths balance across SMs):
@@ -418,7 +418,7 @@ static int plan(dhmc_handle* h) {
   h->scratch_per_cta = (size_t)(h->n_slots - h->n_sm) * slot_doubles;
   cudaFree(h->scratch); h->scratch = nullptr;
   CK(cudaMalloc(&h->scratch, sizeof(double) * h->scratch_per_cta * (size_t)h->grid * (size_t)G));
-  // (an access-policy window over the slot arena was measured and rejected: 1.10e8 vs 1.17e8 leapfrog-steps/s at C2)
+  // (an access-policy window over the slot arena was tried and rejected: slower at C2)
   if (h->lN) {   // residual scratch of the logistic family follows the grid
     cudaFree(h->lr); h->lr = nullptr;
     CK(cudaMalloc(&h->lr, sizeof(double) * (size_t)h->lN * lr_rows(h)));
@@ -708,9 +708,8 @@ int dhmc_create(const dhmc_config* cfg, dhmc_handle** out) {
   k_fill<<<1024, 256, 0, h->stream>>>(h->minv, 1.0, B * D);   // κ = GaussianKineticEnergy(D), mcmc.jl:130
   h->launches += 1;
 
-  // Opt-in (DHMC_L2_WINDOW=1): persisting-L2 window over the logistic design matrix.  Measured on the B200: no gain for C4
-  // (the matrix stays L2-resident anyway), and the carve-out costs the other kernels L2 capacity (C2: 1.17e8 -> 1.09e8
-  // leapfrog-steps/s, streaming leapfrog 0.96 -> 0.42 of the HBM peak), hence off by default.
+  // Opt-in (DHMC_L2_WINDOW=1): persisting-L2 window over the logistic design matrix.  Off by default: the 20 MB matrix of C4
+  // stays L2-resident anyway, and the carve-out costs the other kernels L2 capacity.
   if (std::getenv("DHMC_L2_WINDOW") && std::atoi(std::getenv("DHMC_L2_WINDOW")) == 1) {
     h->l2_persist_max = (size_t)prop.persistingL2CacheMaxSize;
     h->l2_window_max = (size_t)prop.accessPolicyMaxWindowSize;

@@ -1,4 +1,4 @@
-// kernels.cuh — the sm_100a kernels of the many-chain NUTS engine (templates; instantiated per
+// kernels.cuh — the sm_90a kernels of the many-chain NUTS engine (templates; instantiated per
 // log-density family in family_tu.cu, looked up by the host side in dhmc_b200.cu).
 //
 // Kernels (one chain group of T threads = one CTA; persistent, chains pulled

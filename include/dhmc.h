@@ -1,9 +1,9 @@
-/* dhmc.h — C ABI of the B200-native many-chain NUTS engine (libdhmc_b200.so).
+/* dhmc.h — C ABI of the H100-native many-chain NUTS engine (libdhmc_b200.so).
  *
  * Drop-in boundary for the sampler path of tpapp/DynamicHMC.jl (SURVEY.md §8b):
  * host code (Julia via ccall, or the Python mirror in dynamichmc.jl_b200/)
  * keeps the mcmc_with_warmup / LogDensityProblems surface and calls these entry
- * points; everything numeric runs in hand-written sm_100a CUDA.  Plain pointers
+ * points; everything numeric runs in hand-written sm_90a CUDA.  Plain pointers
  * and sizes only.  All functions return a status (0 = ok) unless noted.
  *
  * Conventions

@@ -1,5 +1,5 @@
 /* dhmc_math.h — deterministic scalar math + counter-based RNG shared by the
- * sm_100a kernels (dynamichmc.jl_b200/csrc) and the CPU oracle (oracle/).
+ * sm_90a kernels (dynamichmc.jl_b200/csrc) and the CPU oracle (oracle/).
  *
  * Why this header exists: the parity gate (SURVEY.md §8d) wants the INTEGER
  * decisions of the NUTS tree (depth, termination, steps, accept bits) bit-exact
@@ -8,7 +8,7 @@
  * IEEE-754 operations on both sides.  libm (glibc) and libdevice differ in the
  * last ulp, so exp/log/log1p/sincos are written here once, using only
  * + - * / sqrt fma and integer bit operations, all of which are correctly
- * rounded on x86-64 and on sm_100a.  Build rules: g++ -ffp-contract=off -mfma,
+ * rounded on x86-64 and on sm_90a.  Build rules: g++ -ffp-contract=off -mfma,
  * nvcc -fmad=false.  fma() is used explicitly where a fused operation is wanted.
  *
  * The RNG is Philox-4x32-10 (Salmon et al. 2011), keyed by the user seed and

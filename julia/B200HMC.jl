@@ -86,7 +86,7 @@ the header's formulas receive; `cpu` optionally is `q -> (ℓ(q), ∇ℓ(q))` fo
 A user-model library carries the USER family only, and `LIB` is a per-module constant, so such a model is run through a copy
 of this module bound to its library:
 
-    lib = B200HMC.compile_user_model("include/models/rosenbrock.h")       # make user USER_HEADER=… (nvcc, sm_100a)
+    lib = B200HMC.compile_user_model("include/models/rosenbrock.h")       # make user USER_HEADER=… (nvcc, sm_90a)
     M = B200HMC.bind_user_library(lib)                                     # a copy of B200HMC with LIB = lib
     results = M.mcmc_with_warmup(2026, M.UserModel(100, [1.0, 5.0]), 100; chains = 65_536)
 """

@@ -1,4 +1,4 @@
-# parity.jl — pin the B200 engine against the REAL DynamicHMC.jl (run where Julia + DynamicHMC are installed; a GPU is
+# parity.jl — pin the CUDA engine against the REAL DynamicHMC.jl (run where Julia + DynamicHMC are installed; a GPU is
 # needed only for the device half).  Not executed in the build image (no Julia there): it exists so that a maintainer can
 # close the "parity unpinned" items of SURVEY.md §8c — Julia's Random stream, LogExpFunctions.logaddexp, BLAS dot order.
 #

@@ -4,6 +4,7 @@ the timed loops, the auxiliary legs, the reductions and the one JSON line on std
 (tests/test_bench_contract.py).  Numbers printed under it mean nothing."""
 import os
 import sys
+import types
 
 import numpy as np
 
@@ -15,6 +16,8 @@ import torch  # noqa: E402
 torch.cuda.is_available = lambda: True
 torch.cuda.set_device = lambda *_a, **_k: None
 torch.cuda.synchronize = lambda *_a, **_k: None
+torch.cuda.get_device_properties = lambda *_a, **_k: types.SimpleNamespace(name="stub", multi_processor_count=132,
+                                                                           L2_cache_size=50 << 20)
 _empty, _tensor = torch.empty, torch.tensor
 torch.empty = lambda *a, device=None, **k: _empty(*a, **k)
 torch.tensor = lambda *a, device=None, **k: _tensor(*a, **k)

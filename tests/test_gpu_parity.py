@@ -585,7 +585,7 @@ def test_logistic_packed_groups_equal_one_chain_per_cta(pkg, N, p, K, M):
                                             (1037, 77, 19, 0, "Symmetric"), (31, 5, 8, 0, "Symmetric"),
                                             (700, 200, 10, 0, "Symmetric"), (640, 256, 9, 2, "Symmetric")])
 def test_logistic_mma_likelihood_equals_fma_loops(pkg, monkeypatch, N, p, K, warps, M):
-    """mma.sync.m8n8k4.f64 accumulates as sequential FMAs (profiles/r01_dmma_order_probe.txt), so the
+    """mma.sync.m8n8k4.f64 accumulates as sequential FMAs (benchmarks/dmma_order_probe.cu), so the
     tensor-core / TMA formulation (the default of packed chain groups: likelihood rounds and, with a Symmetric
     metric, the cooperative M⁻¹p) must reproduce the FMA formulation bit for bit — odd dimensions, ragged last
     row block, one or two warps per chain, chains that run out early."""

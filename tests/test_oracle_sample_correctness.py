@@ -6,7 +6,7 @@ with the reference's thresholds.  Targets that need a dense covariance or a mixt
 oracle (include/models/mvnormal_dense.h, mixture_normals.h — the LogDensityTestSuite constructions `multivariate_normal(μ, L)`
 and `mix(α, ℓ₁, ℓ₂)`), with dense adaptation `default_warmup_stages(; M = Symmetric)` (MCMC_ARGS2, :12) where the reference
 uses it, and the reference's two-pass window (co)variance (welford=False).  LogDensityTestSuite's `elongate` / `funnel()`
-transforms are absent from /root/reference (un-vendored dependency), so those three testsets are not ported."""
+transforms are absent from the reference (un-vendored dependency), so those three testsets are not ported."""
 import os
 
 import numpy as np

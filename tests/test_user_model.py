@@ -4,7 +4,7 @@ model header contract"; examples in include/models/) compiled into its own build
 
 CPU part: the oracle built from the same header — (i) Neal's funnel written as a user model reproduces the shipped FUNNEL
 family bit for bit (values, trees, whole warm-ups), which pins the user-model evaluation order to a shipped one; (ii) the
-example models' ℓ, ∇ℓ against numpy closed forms and finite differences; (iii) the user-model library builds for sm_100a,
+example models' ℓ, ∇ℓ against numpy closed forms and finite differences; (iii) the user-model library builds for sm_90a,
 exports the whole C ABI and reports its model, while the stock library refuses family 4.
 GPU part (-m gpu): the CUDA path of a user model against that oracle, bit for bit, and against the shipped family."""
 import ctypes as C
@@ -158,7 +158,7 @@ def test_model_without_sums_oracle_values(po):
 
 # ------------------------------------------------------------------ CPU: the user-model build of the library
 def test_user_library_builds_and_reports_its_model(pkg):
-    """nvcc cross-compiles the model for sm_100a (no GPU needed); the result carries the whole C ABI plus the model."""
+    """nvcc cross-compiles the model for sm_90a (no GPU needed); the result carries the whole C ABI plus the model."""
     so = pkg.compile_user_model(_hdr("rosenbrock"), deep=True)        # the build __graft_entry__.build() prepares
     lib = pkg._lib.lib(so)
     for name in pkg._lib.EXPORTS:
