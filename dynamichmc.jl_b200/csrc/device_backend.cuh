@@ -1,7 +1,7 @@
 // device_backend.cuh — sm_90a vector backend of the NUTS state machine.
 //
 // One chain = one chain group of T = 32·W threads (= one CTA; packed chain groups of the
-// logistic family put 8 groups in a CTA, see coop_core).  Element i of
+// logistic family put 8 groups in a CTA, see coop_core_tma).  Element i of
 // every D-vector belongs to thread (i mod T), register slot e = i div T, so a
 // vector is EPL doubles per thread, HBM accesses of a chain row are fully
 // coalesced, shared-memory slot accesses are conflict-free, and — because the
@@ -65,225 +65,15 @@ __host__ __device__ inline SmemLayout smem_layout(int W, int n_sm, size_t stride
   return L;
 }
 
-// ---- packed chain groups (logistic family): one likelihood round of a whole CTA ----
-// Every warp of the CTA calls this the same number of times: a warp with a chain calls it
-// from eval_model (active, its β already published in cb_beta), a warp that has run out of
-// chains attends from coop_finish until all warps are done, so the CTA barriers below
-// always see all 32·G threads.
-//   phase 1:  rows n are split over all threads (four per thread and pass); a thread computes
-//             η_n of all G chains, then the ll term and the residual per chain;
-//   phase 1b: each active warp sums its chain's ll terms in the lane-strided order;
-//   phase 2:  columns j are split over the threads; a thread accumulates (Xᵀr)_j of all G
-//             chains over n = 0..N-1.
-// Both passes over the design matrix (Xᵀ in phase 1, X in phase 2) are fed through a
-// three-stage cp.async ring in shared memory: each element of X reaches the SM once per G
-// gradients and two tiles are always in flight, so neither L2 nor HBM latency is exposed.
-// Returns false when no warp is active any more (every warp is done); otherwise true with this
-// lane's partial Σ ll in *sll_out.  Requires D <= 32·G.
-constexpr int kCoopStages = 3;
-constexpr int kCoopTile = 4096;                                       // doubles of X / Xᵀ per stage
-constexpr int kCoopMaxRows = 64;                                      // rows of X per phase-2 tile, at most
-__host__ __device__ constexpr int coop_stage_doubles(int G) { return kCoopTile + kCoopMaxRows * G; }   // + residuals [rows][G]
-__host__ __device__ inline int coop_rows(int D) {                     // even, rows·D <= kCoopTile (D <= 256)
-  int r = (kCoopTile / (D < 1 ? 1 : D)) & ~1;
-  return r < 2 ? 2 : r > kCoopMaxRows ? kCoopMaxRows : r;
-}
-__device__ __forceinline__ void cp_async16(void* dst_smem, const void* src) {
-  const unsigned d = (unsigned)__cvta_generic_to_shared(dst_smem);
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(src) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-
-// lXt has leading dimension ldn (even, >= N); lres is [N][G] (row-major), lll is [G][N].
-// A chain group is W warps (T = 32·W threads: tid within the group, grp = group within the CTA).
-template <int G, int W>
-__device__ __noinline__ bool coop_core(double* sll_out, bool active, int tid, int grp, int ctid, int D, int lN, int ldn,
-                                         const double* __restrict__ lX, const double* __restrict__ lXt,
-                                         const double* __restrict__ ly, double* lres, double* lll,
-                                         int* cb_flags, const double* cb_beta, double* cb_grad, double* cb_stage) {
-  constexpr int T = 32 * W;
-  constexpr int NT = T * G;                // threads of the CTA
-  constexpr int NC = 32 * G;               // columns handled per pass of phase 2 (D <= NC)
-  constexpr int S = kCoopStages;
-  constexpr int STG = coop_stage_doubles(G);
-  if (tid == 0) cb_flags[grp] = active ? 1 : 0;
-  __syncthreads();
-  unsigned amask = 0;
-#pragma unroll
-  for (int gg = 0; gg < G; ++gg)
-    if (cb_flags[gg]) amask |= 1u << gg;
-  if (amask == 0) return false;        // no warp has a chain any more: every warp is done
-
-  // ---------------- phase 1: tiles of J rows of Xᵀ × RB observations
-  {
-    constexpr int U = 4 / W;               // observations per thread and pass
-    constexpr int RB = U * NT;             // observations per pass
-    constexpr int J = kCoopTile / RB;      // coefficients per tile
-    static_assert(U >= 1 && J >= 1 && J * RB == kCoopTile, "tile shape");
-    const int nchunks = (D + J - 1) / J;
-    const int npass = (lN + RB - 1) / RB;
-    const int ntiles = npass * nchunks;
-    auto issue = [&](int t) {
-      if (t < ntiles) {
-        const int ps = t / nchunks, ch = t - ps * nchunks;
-        const int n0 = ps * RB;
-        const int cnt = ldn - n0 < RB ? ldn - n0 : RB;     // doubles per row segment (even)
-        const int cpr = cnt >> 1;                           // 16-byte pieces per row segment
-        double* dst = cb_stage + (size_t)(t % S) * STG;
-#pragma unroll
-        for (int jj = 0; jj < J; ++jj) {
-          const int j = ch * J + jj;
-          if (j < D) {
-            const double* sj = lXt + (size_t)j * ldn + n0;
-            for (int k = ctid; k < cpr; k += NT) cp_async16(dst + jj * RB + 2 * k, sj + 2 * k);
-          }
-        }
-      }
-      cp_async_commit();                   // always: group counting stays uniform
-    };
-    issue(0);
-    issue(1);
-    static_assert(DHMC_LOGIT_CHUNK % J == 0, "η chunks are whole tiles");
-    double eta[U][G], etot[U][G];          // running chunk sum, sum of the finished chunks (dhmc_logit_eta)
-    for (int t = 0; t < ntiles; ++t) {
-      cp_async_wait<1>();                  // this thread's pieces of tile t have landed
-      __syncthreads();                     // everyone's have, and everyone is done with tile t-1
-      issue(t + 2);                        // refills the stage of tile t-1
-      const int ps = t / nchunks, ch = t - ps * nchunks;
-      if ((ch * J) % DHMC_LOGIT_CHUNK == 0) {
-#pragma unroll
-        for (int u = 0; u < U; ++u)
-#pragma unroll
-          for (int gg = 0; gg < G; ++gg) {
-            if (ch != 0) etot[u][gg] = (ch * J == DHMC_LOGIT_CHUNK) ? eta[u][gg] : etot[u][gg] + eta[u][gg];
-            eta[u][gg] = 0.0;
-          }
-      }
-      const double* src = cb_stage + (size_t)(t % S) * STG + ctid;
-#pragma unroll
-      for (int jj = 0; jj < J; ++jj) {
-        const int j = ch * J + jj;
-        if (j < D) {
-          double x[U];
-#pragma unroll
-          for (int u = 0; u < U; ++u) x[u] = src[jj * RB + u * NT];
-          const double* bj = cb_beta + (size_t)j * G;
-#pragma unroll
-          for (int gg = 0; gg < G; ++gg) {
-            const double bv = bj[gg];
-#pragma unroll
-            for (int u = 0; u < U; ++u) eta[u][gg] = dhmc_logit_mac(eta[u][gg], x[u], bv);
-          }
-        }
-      }
-      if (ch == nchunks - 1) {
-        const bool one_chunk = D <= DHMC_LOGIT_CHUNK;
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-          const int n = ps * RB + ctid + u * NT;
-          if (n < lN) {
-            const double yn = __ldg(ly + n);
-#pragma unroll
-            for (int gg = 0; gg < G; ++gg) {
-              if (amask & (1u << gg)) {
-                double llv, rv;
-                const double etav = one_chunk ? eta[u][gg] : etot[u][gg] + eta[u][gg];
-                dhmc_logit_ll_resid(yn, etav, &llv, &rv);
-                lll[(size_t)gg * lN + n] = llv;
-                lres[(size_t)n * G + gg] = rv;
-              }
-            }
-          }
-        }
-      }
-    }
-    cp_async_wait<0>();
-    __syncthreads();
-  }
-  // ---------------- phase 1b: thread v of the group sums n = v, v+T, … (the canonical partials)
-  double sll = 0.0;
-  if (active) {
-    const double* t = lll + (size_t)grp * lN;
-    for (int n = tid; n < lN; n += T) sll = sll + t[n];
-  }
-  // ---------------- phase 2: tiles of R rows of X with their residuals [R][G]; thread = (column j,
-  // set of GH chains): with two warps per chain the two halves of the CTA take half the chains each
-  {
-    constexpr int GH = G / W;
-    static_assert(GH * W == G, "chains split evenly over the column sets");
-    const int col = ctid % NC, g0 = (ctid / NC) * GH;
-    const int R = coop_rows(D);
-    const int ntiles = (lN + R - 1) / R;
-    auto issue = [&](int t) {
-      if (t < ntiles) {
-        const int n0 = t * R;
-        const int rows = lN - n0 < R ? lN - n0 : R;
-        double* dst = cb_stage + (size_t)(t % S) * STG;
-        const double* sx = lX + (size_t)n0 * D;            // 16-byte aligned: R is even
-        const int cx = (rows * D + 1) >> 1;                 // X is allocated with two doubles of slack
-        for (int c = ctid; c < cx; c += NT) cp_async16(dst + 2 * c, sx + 2 * c);
-        const double* sr = lres + (size_t)n0 * G;
-        const int cr = (rows * G) >> 1;
-        for (int c = ctid; c < cr; c += NT) cp_async16(dst + kCoopTile + 2 * c, sr + 2 * c);
-      }
-      cp_async_commit();
-    };
-    issue(0);
-    issue(1);
-    double acc[GH];
-#pragma unroll
-    for (int gg = 0; gg < GH; ++gg) acc[gg] = 0.0;
-    for (int t = 0; t < ntiles; ++t) {
-      cp_async_wait<1>();
-      __syncthreads();
-      issue(t + 2);
-      const int n0 = t * R;
-      const int rows = lN - n0 < R ? lN - n0 : R;
-      if (col < D) {
-        // rows in increasing n; operands are fetched from shared memory one row ahead of their use
-        const double* xr = cb_stage + (size_t)(t % S) * STG + col;
-        const double* rr = cb_stage + (size_t)(t % S) * STG + kCoopTile + g0;
-        double r0[GH], r1[GH];
-        double x0 = 0.0, x1 = 0.0;
-#define DHMC_COOP_LD(r, x, nn)                                   \
-        if ((nn) < rows) {                                       \
-          x = xr[(size_t)(nn) * D];                              \
-          _Pragma("unroll") for (int gg = 0; gg < GH; ++gg) r[gg] = rr[(nn) * G + gg]; \
-        }
-#define DHMC_COOP_ACC(r, x, nn)                                  \
-        if ((nn) < rows) {                                       \
-          _Pragma("unroll") for (int gg = 0; gg < GH; ++gg) acc[gg] = dhmc_logit_mac(acc[gg], x, r[gg]); \
-        }
-        DHMC_COOP_LD(r0, x0, 0)
-        for (int nn = 0; nn < rows; nn += 2) {
-          DHMC_COOP_LD(r1, x1, nn + 1)
-          DHMC_COOP_ACC(r0, x0, nn)
-          DHMC_COOP_LD(r0, x0, nn + 2)
-          DHMC_COOP_ACC(r1, x1, nn + 1)
-        }
-#undef DHMC_COOP_LD
-#undef DHMC_COOP_ACC
-      }
-    }
-    cp_async_wait<0>();
-    __syncthreads();                       // cb_grad lives in stage 0 of the ring: everyone is done with the tiles
-    if (col < D) {
-#pragma unroll
-      for (int gg = 0; gg < GH; ++gg) cb_grad[(size_t)(g0 + gg) * NC + col] = acc[gg];
-    }
-    __syncthreads();
-  }
-  *sll_out = sll;
-  return true;
-}
-
-// ---- the likelihood round on the FP64 tensor cores, fed by TMA bulk copies (default for packed groups) ----
+// ---- packed chain groups (logistic family): one likelihood round of the whole CTA on the FP64 tensor cores ----
+// Every warp of the CTA calls this the same number of times: a warp with a chain calls it from eval_model
+// (active, its β already published), a warp that has run out of chains attends from coop_finish until all
+// warps are done, so the CTA barriers below always see all 32·G threads.
 // mma.sync.m8n8k4.f64 (SASS DMMA.8x8x4) computes fma(a3,b3, fma(a2,b2, fma(a1,b1, fma(a0,b0, c))))
-// (benchmarks/dmma_order_probe.cu; test_logistic_mma_likelihood_equals_fma_loops holds the kernels to it),
-// i.e. the model's own sequential order, so the results are those of coop_core bit for bit.  On the H100
-// the DMMA pipe has twice the DFMA rate (data sheet) with 1/8 of the instructions.
+// (benchmarks/dmma_order_probe.cu), i.e. the model's own sequential order, so the results are those of the
+// one-chain-per-CTA FMA loops (eval_model) bit for bit; test_logistic_packed_groups_equal_one_chain_per_cta
+// holds the kernels to it.  On the H100 the DMMA pipe has twice the DFMA rate (data sheet) with 1/8 of the
+// instructions.
 //
 // One pass over the design matrix per gradient.  X is kept in HBM/L2 as zero-padded row blocks
 // [32 rows][XS] (XS ≡ 4 mod 16 doubles: every fragment load below is bank-conflict free); one elected
@@ -402,11 +192,11 @@ __device__ __forceinline__ void mma_chunk_2tiles(uint32_t ap, uint32_t ap2, uint
 // blocked dot product dm_blocked_dot), the chunk sums of all rows are collected in shared memory and added in order when
 // the chain's last block is done.  x is published in the β area [chain][kTmaBS] and y handed back in place.
 // Returns false when no warp of the CTA is active any more.
-template <int G, int W>
+template <int G>
 __device__ __noinline__ bool coop_matvec_tma(bool active, long chain, int tid, int grp, int ctid, int D,
                                              const double* __restrict__ Mp, unsigned char* shared, uint32_t& ring_n) {
-  constexpr int NT = 32 * W * G;
-  constexpr int NW = W * G;
+  constexpr int NT = 32 * G;
+  constexpr int NW = G;
   constexpr int MW = 8;
   int* cb_flags = reinterpret_cast<int*>(shared);
   int* cb_chain = reinterpret_cast<int*>(shared + 32);        // [G] chain index of every group (metric lookup)
@@ -498,11 +288,11 @@ __device__ __noinline__ bool coop_matvec_tma(bool active, long chain, int tid, i
 // semantics): M⁻¹·[x₀ … x₇] is a true GEMM — the metric streams through the ring ONCE per product (not once per chain), and
 // the MMA's n-dimension carries the eight chains' vectors exactly as in the likelihood's P1.  Per 32-row block: P1 (chunk
 // sums of two row tiles per warp) → barrier → 256 lanes add the chunk sums in order → y [chain][row].
-template <int G, int W>
+template <int G>
 __device__ __noinline__ bool coop_matmul_pooled_tma(bool active, long chain, int tid, int grp, int ctid, int D,
                                                     const double* __restrict__ Mp, unsigned char* shared, uint32_t& ring_n) {
-  constexpr int NT = 32 * W * G;
-  constexpr int NW = W * G;
+  constexpr int NT = 32 * G;
+  constexpr int NW = G;
   constexpr int MW = 8;
   int* cb_flags = reinterpret_cast<int*>(shared);
   int* cb_chain = reinterpret_cast<int*>(shared + 32);
@@ -586,28 +376,15 @@ __device__ __noinline__ bool coop_matmul_pooled_tma(bool active, long chain, int
   return true;
 }
 
-// optional cycle accounting of the round's phases (build with -DDHMC_PROFILE_ROUNDS; variants/ only)
-#ifdef DHMC_PROFILE_ROUNDS
-#define DHMC_PROF_DECL long long pf_t = clock64(), pf_acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-#define DHMC_PROF(i) do { const long long t_ = clock64(); pf_acc[i] += t_ - pf_t; pf_t = t_; } while (0)
-#define DHMC_PROF_FLUSH(ptr) do { if (ptr) { for (int i_ = 0; i_ < 8; ++i_) (ptr)[i_] += (unsigned long long)pf_acc[i_]; (ptr)[8] += 1; } } while (0)
-#else
-#define DHMC_PROF_DECL
-#define DHMC_PROF(i) do { } while (0)
-#define DHMC_PROF_FLUSH(ptr) do { } while (0)
-#endif
-
-// lXp: padded row blocks of X, [nblk·32][XS]; lll: unused (the FMA formulation's global ll scratch);
-// shared: the CTA-shared area (layout above); ring_n: blocks streamed so far (same in all threads).
-template <int G, int W>
+// lXp: padded row blocks of X, [nblk·32][XS]; shared: the CTA-shared area (layout above);
+// ring_n: blocks streamed so far (same in all threads).  Returns false when no warp is active any more;
+// otherwise true with this lane's partial Σ ll in *sll_out.
+template <int G>
 __device__ __noinline__ bool coop_core_tma(double* sll_out, bool active, int tid, int grp, int ctid, int D, int lN,
-                                           const double* __restrict__ lXp, const double* __restrict__ ly, double* lll,
-                                           unsigned char* shared, uint32_t& ring_n, unsigned long long* prof) {
+                                           const double* __restrict__ lXp, const double* __restrict__ ly,
+                                           unsigned char* shared, uint32_t& ring_n) {
   static_assert(G == 8, "the n-dimension of the MMA is the chain");
-  DHMC_PROF_DECL
-  constexpr int T = 32 * W;
-  constexpr int NT = T * G;
-  constexpr int NW = W * G;                 // warps of the CTA
+  constexpr int NW = G;                     // warps of the CTA, one per chain
   constexpr int MW = 8;                     // warps that issue DMMAs (two per sub-partition saturate the pipe; more only add
                                             // shared-memory traffic: operands are reused across a warp's tiles)
   constexpr int JT = 32 / MW;               // coefficient tiles per MMA warp in P2 (D <= 256)
@@ -627,7 +404,6 @@ __device__ __noinline__ bool coop_core_tma(double* sll_out, bool active, int tid
   const int fr = lane >> 2, fk = lane & 3;  // fragment row / k index of this lane
   if (tid == 0) cb_flags[grp] = active ? 1 : 0;
   __syncthreads();                          // β and flags are published; the ring (last round's Xᵀr) is free
-  DHMC_PROF(0);                             // 0: waiting for the other chains to arrive
   unsigned amask = 0;
 #pragma unroll
   for (int gg = 0; gg < G; ++gg)
@@ -664,9 +440,7 @@ __device__ __noinline__ bool coop_core_tma(double* sll_out, bool active, int tid
   double acc[JT][2];
 #pragma unroll
   for (int q = 0; q < JT; ++q) { acc[q][0] = 0.0; acc[q][1] = 0.0; }
-  double sl[W];                             // E: this lane's Σ ll partials = those of threads lane, lane+32 of chain wq
-#pragma unroll
-  for (int hh = 0; hh < W; ++hh) sl[hh] = 0.0;
+  double sl = 0.0;                          // E: this lane's Σ ll partial (thread `lane` of chain wq)
   // P1 work of an MMA warp: chunk c = wq & 3, row tiles 2·(wq >> 2) and 2·(wq >> 2) + 1 (they share the β fragments)
   const int pc1 = wq & 3, mp = (wq >> 2) & 1;
   const uint32_t p1_a = (uint32_t)(sizeof(double) * ((16 * mp + fr) * XS + fk));     // A fragment of P1 within a stage (second tile: + 8 rows)
@@ -683,7 +457,6 @@ __device__ __noinline__ bool coop_core_tma(double* sll_out, bool active, int tid
     // chain of up to 16 DMMAs per chunk (26 clk each), fragments fetched one group of four k-steps ahead;
     // k-steps beyond ⌈D/4⌉ hit the zero padding of X and β (16·⌈D/16⌉ <= XS)
     mbar_wait(full + s, par);
-    DHMC_PROF(1);                           // 1: waiting for the block
     if (wq < MW) {
       const int g0 = 4 * pc1, g1 = (4 * pc1 + 4 < ng) ? 4 * pc1 + 4 : ng;    // k-step groups of this chunk
       if (g0 < g1) {
@@ -697,13 +470,11 @@ __device__ __noinline__ bool coop_core_tma(double* sll_out, bool active, int tid
         sts64(ea + (uint32_t)(sizeof(double) * ((2 * fk + 1) * kTmaES + 8)), d1);
       }
     }
-    DHMC_PROF(2);                           // 2: P1 compute
     __syncthreads();
-    DHMC_PROF(3);                           // 3: barrier after P1
     // ---- E: warp gg evaluates chain gg, lane = row: η = ((s₀ + s₁) + s₂) + s₃, ll term into this lane's
-    // canonical partial (thread (n mod T) of the chain sums n, n+T, … in increasing n), residual -> shared tile
-    if (wq >= NW - G) {
-      const int gg = wq - (NW - G), r = lane;
+    // canonical partial (thread (n mod 32) of the chain sums n, n+32, … in increasing n), residual -> shared tile
+    {
+      const int gg = wq, r = lane;
       const int nrow = b * kTmaRows + r;
       const uint32_t ea = eta_a + (uint32_t)(sizeof(double) * (gg * kTmaES + r));
       double eta = lds64(ea);
@@ -712,15 +483,11 @@ __device__ __noinline__ bool coop_core_tma(double* sll_out, bool active, int tid
       if (nrow < lN) {
         double llv;
         dhmc_logit_ll_resid_tabs(__ldg(ly + nrow), eta, &llv, &rv, tabs);
-#pragma unroll
-        for (int hh = 0; hh < W; ++hh)
-          if ((b & (W - 1)) == hh) sl[hh] = sl[hh] + llv;
+        sl = sl + llv;
       }
       sts64(res_a + (uint32_t)(sizeof(double) * (gg * kTmaES + r)), rv);
     }
-    DHMC_PROF(4);                           // 4: E compute
     __syncthreads();
-    DHMC_PROF(5);                           // 5: barrier after E
     // ---- P2: (Xᵀr) += Xᵀ[coefficients × rows of the block] · r; operands one k-step ahead
     if (wq < MW) {
       const uint32_t ap = xt + p2_a;
@@ -749,7 +516,6 @@ __device__ __noinline__ bool coop_core_tma(double* sll_out, bool active, int tid
     if (lane == 0) mbar_arrive(empty + s);
     if (producer && b + 2 < nblk) issue(b + 2);
     __syncwarp();
-    DHMC_PROF(6);                           // 6: P2
   }
   ring_n = n0 + (uint32_t)nblk;
   __syncthreads();                          // every warp is done with the ring and the tiles: hand Xᵀr and Σ ll back
@@ -761,14 +527,9 @@ __device__ __noinline__ bool coop_core_tma(double* sll_out, bool active, int tid
       sts64(ring_a + (uint32_t)(sizeof(double) * ((2 * fk + 1) * XS + j)), acc[q][1]);
     }
   }
-  if (wq >= NW - G) {
-#pragma unroll
-    for (int hh = 0; hh < W; ++hh) sts64(eta_a + (uint32_t)(sizeof(double) * ((wq - (NW - G)) * T + 32 * hh + lane)), sl[hh]);   // [chain][T]
-  }
+  sts64(eta_a + (uint32_t)(sizeof(double) * (wq * 32 + lane)), sl);   // [chain][32]
   __syncthreads();
-  const double sll = active ? lds64(eta_a + (uint32_t)(sizeof(double) * (grp * T + tid))) : 0.0;
-  DHMC_PROF(7);                             // 7: hand-back
-  if (lane == 0) DHMC_PROF_FLUSH(prof ? prof + (size_t)wq * 16 : prof);
+  const double sll = active ? lds64(eta_a + (uint32_t)(sizeof(double) * (grp * 32 + tid))) : 0.0;
   *sll_out = sll;
   return true;
 }
@@ -777,26 +538,23 @@ __device__ __noinline__ bool coop_core_tma(double* sll_out, bool active, int tid
 // streamed from HBM, kept in registers next to p and stored with it — a momentum
 // slot holds the pair (p, p♯), so the state machine's bookkeeping is unchanged.
 //
-// PACK > 1 ("packed chain groups", logistic family, one or two warps per chain): a CTA holds PACK
-// independent chains.  Everything except the likelihood is private to the chain's warps (which
-// meet at a named barrier of their own); the likelihood is evaluated by the whole CTA for all PACK chains at once
+// PACK > 1 ("packed chain groups", logistic family, one warp per chain): a CTA holds PACK
+// independent chains.  Everything except the likelihood is private to the chain's warp; the
+// likelihood is evaluated by the whole CTA for all PACK chains at once on the FP64 tensor cores
 // (coop_round), so every element of X is read once per PACK gradients instead of once per
 // gradient — the family is bound by L2 traffic on X otherwise.  The per-chain arithmetic
 // and its order are unchanged (η_n sequential in j, (Xᵀr)_j sequential in n, Σ ll lane-strided).
-template <int EPL, int FAM, int WARPS, bool DENSE = false, int PACK = 1, bool MMA = false, bool DEEP = false>
+template <int EPL, int FAM, int WARPS, bool DENSE = false, int PACK = 1, bool DEEP = false>
 struct DeviceBackend {
   static constexpr bool kDeep = DEEP;     // max_depth > 12: the slot pool spills past its register word (nuts_machine.cuh)
-  static constexpr bool kMma = MMA;      // likelihood rounds on the FP64 tensor cores, X streamed by TMA (packed groups only)
-  static_assert(PACK == 1 || (WARPS <= 2 && FAM == DHMC_FAMILY_LOGISTIC), "packed groups: one or two warps per chain, logistic family");
+  static_assert(PACK == 1 || (WARPS == 1 && FAM == DHMC_FAMILY_LOGISTIC), "packed groups: one warp per chain, logistic family");
   static constexpr int G = PACK;
   int grp, ctid;                            // warp (= chain group) within the CTA, thread within the CTA
-  int* cb_flags; double* cb_beta; double* cb_grad; double* cb_stage;   // CTA-shared exchange area
-  unsigned char* cb_shared;                 // its base (MMA: layout of tma_smem_bytes)
-  uint32_t ring_n;                          // MMA: blocks of X streamed through the ring so far (uniform over the CTA)
-  const double* lXp;                        // MMA: zero-padded row blocks of X, [⌈N/32⌉·32][tma_xs(D)]
-  unsigned long long* prof;                 // cycle accounting of this CTA ([warp][16]) in profiling builds, else null
-  const double* Mp;                         // MMA + Symmetric metric: padded M⁻¹ of all chains, [chain][⌈D/32⌉·32][tma_xs(D)]
-  double* lll;                              // per-CTA scratch [G][N]: log-likelihood terms (lr holds residuals)
+  double* cb_beta; double* cb_grad;         // CTA-shared exchange area: β [chain][kTmaBS], Xᵀr [chain][tma_xs(D)]
+  unsigned char* cb_shared;                 // its base (layout of tma_smem_bytes)
+  uint32_t ring_n;                          // blocks of X streamed through the ring so far (uniform over the CTA)
+  const double* lXp;                        // zero-padded row blocks of X, [⌈N/32⌉·32][tma_xs(D)]
+  const double* Mp;                         // Symmetric metric: padded M⁻¹ of all chains, [chain][⌈D/32⌉·32][tma_xs(D)]
   // geometry: T = 32·WARPS threads per chain, compile-time so that strides fold
   static constexpr int W = WARPS;
   static constexpr int T = 32 * WARPS;
@@ -973,10 +731,9 @@ struct DeviceBackend {
   }
   __device__ __forceinline__ Entry get_entry(int j) const { return ctl[j]; }
 
-  // all threads of the chain: the CTA barrier, or — packed groups — named barrier 1 + grp
+  // all threads of the chain: the warp, or the CTA
   __device__ __forceinline__ void group_sync() const {
     if constexpr (W == 1) __syncwarp();
-    else if constexpr (PACK > 1) asm volatile("bar.sync %0, %1;" ::"r"(grp + 1), "n"(32 * WARPS) : "memory");
     else __syncthreads();
   }
   // y = M⁻¹ x for this chain (Symmetric M⁻¹ * v, hamiltonian.jl:110): x is staged in shared
@@ -1118,7 +875,7 @@ struct DeviceBackend {
     return -dm_inf();
   }
 
-  // ---- packed chain groups: one likelihood round of the whole CTA (coop_core above) ----
+  // ---- packed chain groups: one likelihood round of the whole CTA (coop_core_tma above) ----
   // Returns false (attendants only) when every warp of the CTA is done.
   __device__ __forceinline__ bool coop_round(bool active, double& sum_ll, double (&xtr)[EPL]) {
     static_assert(PACK > 1, "packed groups only");
@@ -1126,36 +883,28 @@ struct DeviceBackend {
 #pragma unroll
       for (int e = 0; e < EPL; ++e) {
         const int i = tid + e * T;
-        if (i < D) {
-          if constexpr (MMA) cb_beta[(size_t)grp * kTmaBS + i] = q[e];      // [chain][coefficient]
-          else cb_beta[(size_t)i * G + grp] = q[e];                          // [coefficient][chain]
-        }
+        if (i < D) cb_beta[(size_t)grp * kTmaBS + i] = q[e];      // [chain][coefficient]
       }
     }
     double sll = 0.0;
-    bool more;
-    if constexpr (MMA)
-      more = coop_core_tma<G, W>(&sll, active, tid, grp, ctid, D, lN, lXp, ly, lll, cb_shared, ring_n, prof);
-    else
-      more = coop_core<G, W>(&sll, active, tid, grp, ctid, D, lN, lLd, lX, lXt, ly, lr, lll,
-                             cb_flags, cb_beta, cb_grad, cb_stage);
-    if (!more) return false;             // explicit flag (uniform over the CTA), not a property of the data
+    if (!coop_core_tma<G>(&sll, active, tid, grp, ctid, D, lN, lXp, ly, cb_shared, ring_n))
+      return false;                      // explicit flag (uniform over the CTA), not a property of the data
     sum_ll = sll;
     if (active) {
 #pragma unroll
       for (int e = 0; e < EPL; ++e) {
         const int i = tid + e * T;
-        xtr[e] = i < D ? cb_grad[(size_t)grp * (MMA ? tma_xs(D) : 32 * G) + i] : 0.0;
+        xtr[e] = i < D ? cb_grad[(size_t)grp * tma_xs(D) + i] : 0.0;
       }
     }
     return true;
   }
-  // packed groups, Symmetric metric, tensor-core build: y = M⁻¹x of all chains of the CTA (coop_matvec_tma)
-  static constexpr bool kCoopMatvec = DENSE && PACK > 1 && MMA;
+  // packed groups, Symmetric metric: y = M⁻¹x of all chains of the CTA (coop_matvec_tma)
+  static constexpr bool kCoopMatvec = DENSE && PACK > 1;
   int pooled;                               // the dense metric is shared by the CTA's 8 chains (DHMC_METRIC_SYMMETRIC_POOLED)
   __device__ __forceinline__ bool coop_matvec_call(bool act) {
-    if (pooled) return coop_matmul_pooled_tma<G, W>(act, chain, tid, grp, ctid, D, Mp, cb_shared, ring_n);
-    return coop_matvec_tma<G, W>(act, chain, tid, grp, ctid, D, Mp, cb_shared, ring_n);
+    if (pooled) return coop_matmul_pooled_tma<G>(act, chain, tid, grp, ctid, D, Mp, cb_shared, ring_n);
+    return coop_matvec_tma<G>(act, chain, tid, grp, ctid, D, Mp, cb_shared, ring_n);
   }
   __device__ __forceinline__ void coop_matvec(const double (&x)[EPL], double (&y)[EPL]) {
 #pragma unroll

@@ -9,8 +9,8 @@
 //   k_eval      evaluate_ℓ(strict) / random_position          hamiltonian.jl:202-217, mcmc.jl:108
 //   k_phase     logdensity(H, z)                              hamiltonian.jl:251-256
 // Logistic family, dim <= 256: k_nuts / k_search run as "packed chain groups" — 8 chains per
-// CTA, each with its own warps and state machine, the likelihood evaluated by the whole CTA
-// (device_backend.cuh: coop_core).
+// CTA, one warp and state machine each, the likelihood evaluated by the whole CTA on the FP64
+// tensor cores (device_backend.cuh: coop_core_tma).
 //
 // There is NO CPU fallback: without a CUDA device dhmc_create fails with
 // DHMC_ECUDA and nothing else can be called.
@@ -42,7 +42,7 @@ using namespace dhmc;
 // (hidden: never bound across two copies of the library loaded into one process)
 #define DHMC_TU_LINKAGE __attribute__((weak, visibility("hidden")))
 #define DHMC_DECL_TU(f, p) const void* dhmc_family_kernel_##f##_##p(int W, int epl, int kernel, int dense) DHMC_TU_LINKAGE;
-DHMC_DECL_TU(0, 0) DHMC_DECL_TU(1, 0) DHMC_DECL_TU(2, 0) DHMC_DECL_TU(3, 0) DHMC_DECL_TU(3, 1) DHMC_DECL_TU(3, 2)
+DHMC_DECL_TU(0, 0) DHMC_DECL_TU(1, 0) DHMC_DECL_TU(2, 0) DHMC_DECL_TU(3, 0) DHMC_DECL_TU(3, 1)
 DHMC_DECL_TU(0, 3) DHMC_DECL_TU(1, 3) DHMC_DECL_TU(2, 3) DHMC_DECL_TU(3, 3)
 #undef DHMC_DECL_TU
 extern "C" {
@@ -51,7 +51,7 @@ const void* dhmc_user_family_kernel_3(int W, int epl, int kernel, int dense) DHM
 const char* dhmc_user_family_name_str(void) DHMC_TU_LINKAGE;
 int dhmc_user_family_min_dim(void) DHMC_TU_LINKAGE;
 }
-// part: 0 = one chain per CTA, 1 = packed chain groups with the FMA likelihood, 2 = packed groups on the tensor cores,
+// part: 0 = one chain per CTA, 1 = packed chain groups (likelihood on the tensor cores),
 // 3 = one chain per CTA with max_depth > 12 (persistent kernels only)
 typedef const void* (*family_tu_fn)(int, int, int, int);
 static family_tu_fn family_tu(int fam, int part) {
@@ -61,7 +61,6 @@ static family_tu_fn family_tu(int fam, int part) {
     case 8: return dhmc_family_kernel_2_0;
     case 12: return dhmc_family_kernel_3_0;
     case 13: return dhmc_family_kernel_3_1;
-    case 14: return dhmc_family_kernel_3_2;
     case 3: return dhmc_family_kernel_0_3;
     case 7: return dhmc_family_kernel_1_3;
     case 11: return dhmc_family_kernel_2_3;
@@ -310,7 +309,6 @@ struct dhmc_handle {
   int T = 0, W = 0, EPL = 0;
   int G = 1;                        // chains per CTA of the persistent kernels (packed chain groups)
   bool deep = false;                // max_depth > 12: kernels whose slot pool spills past 64 slots (part 3), one chain per CTA
-  bool coop_mma = false;            // packed groups: likelihood rounds on the FP64 tensor cores, X streamed by TMA
   size_t stride = 0;
   int n_slots = 0, n_sm = 0, grid = 0, sm_count = 0, light_grid = 0;
   int levels = 13, ntab = 64;       // stack entries per warp (max_depth + 1), slot-table entries (>= n_slots)
@@ -353,7 +351,6 @@ struct dhmc_handle {
   ncclComm_t comm = nullptr;        // multi-GPU: one communicator per handle (dhmc_comm_init)
   int comm_nranks = 1, comm_rank = 0;
   double last_comm_ms = 0;
-  size_t l2_persist_max = 0, l2_window_max = 0;   // persisting-L2 carve-out and largest access-policy window of the device
   std::string err;
 };
 
@@ -368,17 +365,16 @@ static std::string g_create_err;
     }                                                                                 \
   } while (0)
 
-static void set_l2_window(dhmc_handle* h, const void* ptr, size_t bytes);
 // a per-chain staging vector in shared memory: mat-vec input (Symmetric metric), β (logistic), the whole position (USER)
 static bool needs_staging(const dhmc_handle* h) {
   return h->minv_dense || h->cfg.family == DHMC_FAMILY_LOGISTIC || h->cfg.family == DHMC_FAMILY_USER;
 }
 static int kernel_part(const dhmc_handle* h, KernelId k, int G);
 
-// rows of N doubles in the logistic scratch: one per CTA of the light kernels, 2·G per CTA
-// (residuals and ll terms of every packed chain) of the persistent kernels
+// rows of N doubles in the logistic scratch (residuals): one per CTA of the light kernels and, with one chain per CTA,
+// of the persistent kernels (packed groups keep theirs in shared memory)
 static size_t lr_rows(const dhmc_handle* h) {
-  return std::max<size_t>((size_t)h->grid * (h->G > 1 ? 2 * (size_t)h->G : 1), (size_t)h->light_grid);
+  return std::max<size_t>(h->G > 1 ? 0 : (size_t)h->grid, (size_t)h->light_grid);
 }
 
 // Plan the persistent kernels for the current metric kind: CTAs per SM (register
@@ -391,7 +387,7 @@ static int plan(dhmc_handle* h) {
   const size_t xs = needs_staging(h) ? h->stride : 0;
   const int G = h->G;
   auto heavy_smem = [&](int n_sm) -> size_t {
-    return G > 1 ? (size_t)G * group_smem_bytes(h->W, n_sm, slot_doubles, xs, h->levels, h->ntab) + coop_smem_bytes(G, h->coop_mma, (int)h->cfg.dim)
+    return G > 1 ? (size_t)G * group_smem_bytes(h->W, n_sm, slot_doubles, xs, h->levels, h->ntab) + tma_smem_bytes(G, (int)h->cfg.dim)
                  : smem_layout(h->W, n_sm, slot_doubles, xs, h->levels, h->ntab).total;
   };
   struct { size_t total; } L0{heavy_smem(0)};
@@ -426,26 +422,10 @@ static int plan(dhmc_handle* h) {
   return DHMC_OK;
 }
 
-// Keep a re-read working set resident in L2 (access-policy window on the compute stream): the design matrix of the
-// logistic family (every SM sweeps it once per gradient; evicted by the metric / co-moment streams otherwise), else the
-// slot arena of the persistent kernels (its dirty lines were written back and re-fetched between tree levels).
-static void set_l2_window(dhmc_handle* h, const void* ptr, size_t bytes) {
-  if (!ptr || !bytes || h->l2_persist_max == 0) return;
-  cudaStreamAttrValue v;
-  std::memset(&v, 0, sizeof v);
-  const size_t win = std::min(bytes, h->l2_window_max);
-  v.accessPolicyWindow.base_ptr = const_cast<void*>(ptr);
-  v.accessPolicyWindow.num_bytes = win;
-  v.accessPolicyWindow.hitRatio = (float)std::min(1.0, 0.9 * (double)h->l2_persist_max / (double)win);
-  v.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-  v.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-  if (cudaStreamSetAttribute(h->stream, cudaStreamAttributeAccessPolicyWindow, &v) != cudaSuccess) cudaGetLastError();
-}
-
 static int kernel_part(const dhmc_handle* h, KernelId k, int G) {
   const bool heavy = (k == K_NUTS || k == K_SEARCH);
   if (heavy && h->deep) return 3;
-  return G > 1 ? (h->coop_mma ? 2 : 1) : 0;
+  return G > 1 ? 1 : 0;
 }
 
 static int ensure_tmp(dhmc_handle* h, size_t doubles) {      // grow-only device scratch shared by the small entry points
@@ -502,14 +482,6 @@ static int launch(dhmc_handle* h, KernelId k, KArgs a, int timing, bool reset_st
     if (reset_steps) CK(cudaMemsetAsync(h->total_steps, 0, sizeof(unsigned long long), h->stream));
   }
   if (timing == 1 || timing == 2) CK(cudaEventRecord(h->ev0, h->stream));
-#ifdef DHMC_PROFILE_ROUNDS
-  unsigned long long* prof_buf = nullptr;
-  if (k == K_NUTS && G > 1) {
-    CK(cudaMalloc(&prof_buf, sizeof(unsigned long long) * (size_t)grid * 32 * 16));
-    CK(cudaMemsetAsync(prof_buf, 0, sizeof(unsigned long long) * (size_t)grid * 32 * 16, h->stream));
-    a.prof = prof_buf;
-  }
-#endif
   {
     const void* fn = lookup_kernel(h->cfg.family, kernel_part(h, k, G), h->W, h->EPL, k, h->dense);
     if (!fn) { h->err = "kernel not built into this library for this layout (max_depth > 12 needs a user-model library built with its deep part: USER_PARTS=\"0 3\" / deep=True)"; return DHMC_EARG; }
@@ -520,30 +492,6 @@ static int launch(dhmc_handle* h, KernelId k, KArgs a, int timing, bool reset_st
     if (e != cudaSuccess) { h->err = std::string("cudaLaunchKernel: ") + cudaGetErrorString(e); return DHMC_ECUDA; }
   }
   h->launches += 1;
-#ifdef DHMC_PROFILE_ROUNDS
-  if (prof_buf) {   // profiling build: dump the per-warp cycle counters of this launch as one JSON line
-    CK(cudaStreamSynchronize(h->stream));
-    std::vector<unsigned long long> hp((size_t)grid * 32 * 16);
-    CK(cudaMemcpy(hp.data(), prof_buf, hp.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-    cudaFree(prof_buf);
-    const char* path = std::getenv("DHMC_PROF_DUMP");
-    if (FILE* f = std::fopen(path ? path : "dhmc_prof.jsonl", "a")) {
-      const int nw = h->T * G / 32;
-      std::fprintf(f, "{\"kernel\": %d, \"grid\": %d, \"warps\": %d, \"dense\": %d, \"sum\": [", (int)k, grid, nw, (int)h->dense);
-      for (int w = 0; w < nw; ++w) {
-        std::fprintf(f, "%s[", w ? ", " : "");
-        for (int i = 0; i < 10; ++i) {
-          unsigned long long sacc = 0;
-          for (int c = 0; c < grid; ++c) sacc += hp[((size_t)c * 32 + w) * 16 + i];
-          std::fprintf(f, "%s%llu", i ? ", " : "", sacc);
-        }
-        std::fprintf(f, "]");
-      }
-      std::fprintf(f, "]}\n");
-      std::fclose(f);
-    }
-  }
-#endif
   if (timing == 1 || timing == 3) CK(cudaEventRecord(h->ev1, h->stream));
   if (timing == 1) return read_timer(h);
   return DHMC_OK;
@@ -640,23 +588,15 @@ int dhmc_create(const dhmc_config* cfg, dhmc_handle** out) {
   const int rt = cfg->threads_per_chain;
   if (rt != 0 && !(rt == 32 || rt == 64 || rt == 128 || rt == 256)) { g_create_err = "threads_per_chain in {0,32,64,128,256}"; return DHMC_EARG; }
   choose_layout(cfg->dim, rt, &T, &EPL);
-  // logistic regression, dim <= 256: kPack chains per CTA (one warp per chain up to dim 128, two
-  // above) sharing every pass over X (packed chain groups); an explicit threads_per_chain keeps
-  // one chain per CTA
+  // logistic regression, dim <= 256: kPack chains per CTA, one warp each (8 elements per lane above dim 128: eight
+  // warps at 255 registers — the tensor-core rounds need only two warps per sub-partition, and the state machine does
+  // not spill), sharing every pass over X (packed chain groups); an explicit threads_per_chain keeps one chain per CTA
   int pack = 1;
   const bool deep = cfg->max_depth > 12;
   if (cfg->family == DHMC_FAMILY_LOGISTIC && rt == 0 && cfg->dim <= 32 * kPack && !deep) {
-    const char* ev = std::getenv("DHMC_PACK");
-    // one warp per chain (8 elements per lane above dim 128): eight warps at 255 registers — the tensor-core rounds
-    // need only two warps per sub-partition, and the state machine does not spill; DHMC_PACK_WARPS=2: two warps per chain
-    const char* evw = std::getenv("DHMC_PACK_WARPS");
-    if (!(evw && std::atoi(evw) == 2) && cfg->dim > 128) { T = 32; EPL = 8; }
-    if (!(ev && std::atoi(ev) == 0) && packed_layout(T / 32, EPL)) pack = kPack;
+    if (cfg->dim > 128) { T = 32; EPL = 8; }
+    pack = kPack;
   }
-  // packed groups evaluate the likelihood on the FP64 tensor cores (coop_core_tma); DHMC_COOP_MMA=0 selects
-  // the FMA formulation (coop_core) — same results bit for bit
-  const char* evm = std::getenv("DHMC_COOP_MMA");
-  const bool coop_mma = pack > 1 && !(evm && std::atoi(evm) == 0);
   if (T == 0 || EPL == 0) { g_create_err = "dim too large for this build (dim <= 32 * threads_per_chain, 32 only for 256 threads: dim <= 8192)"; return DHMC_EARG; }
   int ndev = 0;
   cudaError_t ce = cudaGetDeviceCount(&ndev);
@@ -667,7 +607,7 @@ int dhmc_create(const dhmc_config* cfg, dhmc_handle** out) {
   }
   if (cfg->device < 0 || cfg->device >= ndev) { g_create_err = "bad device ordinal"; return DHMC_EARG; }
   dhmc_handle* h = new dhmc_handle();
-  h->cfg = *cfg; h->T = T; h->W = T / 32; h->EPL = EPL; h->stride = (size_t)T * EPL; h->G = pack; h->coop_mma = coop_mma; h->deep = deep;
+  h->cfg = *cfg; h->T = T; h->W = T / 32; h->EPL = EPL; h->stride = (size_t)T * EPL; h->G = pack; h->deep = deep;
   h->n_slots = slots_needed(cfg->max_depth);
   h->levels = deep ? cfg->max_depth + 1 : kStdLevels;        // deep persistent kernels size their stack / slot table at run time
   h->ntab = deep ? std::max(kStdTab, (h->n_slots + 7) & ~7) : kStdTab;
@@ -708,16 +648,6 @@ int dhmc_create(const dhmc_config* cfg, dhmc_handle** out) {
   k_fill<<<1024, 256, 0, h->stream>>>(h->minv, 1.0, B * D);   // κ = GaussianKineticEnergy(D), mcmc.jl:130
   h->launches += 1;
 
-  // Opt-in (DHMC_L2_WINDOW=1): persisting-L2 window over the logistic design matrix.  Off by default: the 20 MB matrix of C4
-  // stays L2-resident anyway, and the carve-out costs the other kernels L2 capacity.
-  if (std::getenv("DHMC_L2_WINDOW") && std::atoi(std::getenv("DHMC_L2_WINDOW")) == 1) {
-    h->l2_persist_max = (size_t)prop.persistingL2CacheMaxSize;
-    h->l2_window_max = (size_t)prop.accessPolicyMaxWindowSize;
-    if (h->l2_persist_max && cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, h->l2_persist_max) != cudaSuccess) {
-      cudaGetLastError();
-      h->l2_persist_max = 0;
-    }
-  }
   h->smem_sm = (size_t)prop.sharedMemPerMultiprocessor;          // 228 KB
   h->smem_cta_max = (size_t)prop.sharedMemPerBlockOptin;         // 227 KB
   {
@@ -766,8 +696,7 @@ int dhmc_set_problem(dhmc_handle* h, const double* params, size_t n) {
     cudaFree(h->lX); cudaFree(h->lXt); cudaFree(h->ly); cudaFree(h->lr); cudaFree(h->lXp);
     h->lX = h->lXt = h->ly = h->lr = h->lXp = nullptr;
     const size_t ld = (N + 1) & ~(size_t)1;                 // even leading dimension: 16-byte aligned row segments
-    CK(cudaMalloc(&h->lX, sizeof(double) * (N * D + 2)));  // slack for the last 16-byte piece of a tile
-    CK(cudaMemsetAsync(h->lX, 0, sizeof(double) * (N * D + 2), h->stream));
+    CK(cudaMalloc(&h->lX, sizeof(double) * N * D));
     CK(cudaMalloc(&h->lXt, sizeof(double) * ld * D));
     CK(cudaMalloc(&h->ly, sizeof(double) * N));
     CK(cudaMalloc(&h->lr, sizeof(double) * N * lr_rows(h)));
@@ -775,12 +704,11 @@ int dhmc_set_problem(dhmc_handle* h, const double* params, size_t n) {
     CK(cudaMemcpyAsync(h->ly, params + 1 + N * D, sizeof(double) * N, cudaMemcpyHostToDevice, h->stream));
     k_transpose<<<1024, 256, 0, h->stream>>>(h->lX, h->lXt, N, D, ld);
     h->launches += 1;
-    if (h->coop_mma) {   // row blocks [32][XS] with zero padding (rows >= N, columns >= D): one bulk copy per block
+    if (h->G > 1) {   // row blocks [32][XS] with zero padding (rows >= N, columns >= D): one bulk copy per block
       const size_t xs = (size_t)tma_xs((int)D), rows = (N + kTmaRows - 1) / kTmaRows * kTmaRows;
       CK(cudaMalloc(&h->lXp, sizeof(double) * rows * xs));
       k_pad_rows<<<1024, 256, 0, h->stream>>>(h->lX, h->lXp, N, D, rows, xs);
       h->launches += 1;
-      set_l2_window(h, h->lXp, sizeof(double) * rows * xs);
     }
     h->lN = (int)N; h->lLd = (int)ld;
     CK(cudaStreamSynchronize(h->stream));
@@ -834,7 +762,7 @@ static int ensure_dense(dhmc_handle* h) {
   const int fgrid = (int)std::min<size_t>((size_t)h->sm_count * 4, B);
   CK(cudaMalloc(&h->dense_tmp, sizeof(double) * 3 * dd * (size_t)fgrid));
   CK(cudaMemsetAsync(h->wt, 0, sizeof(double) * B * dd, h->stream));
-  if (h->G > 1 && h->coop_mma) {   // [B][⌈D/32⌉·32][XS]: one bulk copy per 32-row block (coop_matvec_tma)
+  if (h->G > 1) {   // [B][⌈D/32⌉·32][XS]: one bulk copy per 32-row block (coop_matvec_tma)
     const size_t rows = ((size_t)h->cfg.dim + kTmaRows - 1) / kTmaRows * kTmaRows;
     CK(cudaMalloc(&h->minv_pad, sizeof(double) * B * rows * (size_t)tma_xs((int)h->cfg.dim)));
   }

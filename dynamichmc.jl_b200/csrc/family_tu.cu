@@ -1,5 +1,6 @@
 // family_tu.cu — instantiates the kernels of ONE log-density family (and one part of it) per
-// translation unit so that the library builds in parallel: nvcc -DDHMC_TU_FAM=<0..3> -DDHMC_TU_PART=<0..2>.
+// translation unit so that the library builds in parallel: nvcc -DDHMC_TU_FAM=<0..3> -DDHMC_TU_PART=<0, 1, 3>
+// (kernels.cuh: kernel_ptr).
 // The host side (dhmc_b200.cu) reaches the kernels through dhmc_family_kernel_<fam>_<part>().
 #include "kernels.cuh"
 

@@ -9,8 +9,8 @@
 //   k_eval      evaluate_ℓ(strict) / random_position          hamiltonian.jl:202-217, mcmc.jl:108
 //   k_phase     logdensity(H, z)                              hamiltonian.jl:251-256
 // Logistic family, dim <= 256: k_nuts / k_search run as "packed chain groups" — 8 chains per
-// CTA, each with its own warps and state machine, the likelihood evaluated by the whole CTA
-// (device_backend.cuh: coop_core_tma on the FP64 tensor cores, coop_core with plain FMAs).
+// CTA, one warp and state machine each, the likelihood evaluated by the whole CTA on the FP64
+// tensor cores (device_backend.cuh: coop_core_tma).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -55,7 +55,7 @@ struct KArgs {
   double *minv_dense, *wt, *covt;   // Symmetric metric: M⁻¹, Wᵀ, co-moments, each [B][D][D]
   int xs_doubles;               // shared-memory staging vector (0 unless the dense arrays exist)
   const double *lX, *lXt, *ly;  // logistic regression data
-  double* lr;                   // logistic scratch: [grid][lN] residuals, or per CTA of packed groups [lN][G] residuals + [G][lN] ll terms
+  double* lr;                   // logistic scratch of one chain per CTA: [grid][lN] residuals (packed groups need none)
   int lN, lLd;                  // observations, leading dimension of Xᵀ (even)
   const double* lXp;            // tensor-core likelihood: zero-padded row blocks of X
   int levels, ntab;             // deep kernels (max_depth > 12) only: stack entries per warp (max_depth + 1), slot-table entries;
@@ -64,7 +64,6 @@ struct KArgs {
   double* mean_out;             // pooled Symmetric stage: the window mean of every chain [B][D] (else null)
   int pooled;                   // the current dense metric is shared by every group of 8 chains (DHMC_METRIC_SYMMETRIC_POOLED)
   const double* minv_pad;       // tensor-core mat-vec: padded M⁻¹ [B][⌈D/32⌉·32][tma_xs(D)]
-  unsigned long long* prof;     // profiling builds (-DDHMC_PROFILE_ROUNDS): [grid][32 warps][16] cycle counters
 };
 
 // Register budget: minimum resident CTAs per SM the compiler must allow for.
@@ -75,21 +74,12 @@ __host__ __device__ constexpr int min_ctas(int W, int EPL) {
   return W == 1 ? 16 : W == 2 ? 8 : W == 4 ? (EPL >= 8 ? DHMC_MINCTAS_W4E8 : 4) : EPL >= 16 ? 1 : 2;
 }
 
-// packed chain groups (G chains per CTA, one per warp): shared-memory bytes of the CTA-wide
-// exchange area behind the G per-group blocks — flags, β [32G][G], cp.async ring (Xᵀr [G][32G] is
-// handed back in stage 0 of the ring, which is idle between two rounds)
-__host__ __device__ constexpr size_t coop_beta_doubles(int G) { return (size_t)32 * G * G; }
-__host__ __device__ constexpr size_t coop_ring_doubles(int G) { return (size_t)kCoopStages * coop_stage_doubles(G); }
-// mma: the tensor-core / TMA likelihood (device_backend.cuh: coop_core_tma), whose ring depends on dim
-__host__ __device__ inline size_t coop_smem_bytes(int G, bool mma, int D) {
-  return mma ? tma_smem_bytes(G, D) : 64 + sizeof(double) * (coop_beta_doubles(G) + coop_ring_doubles(G));
-}
 __host__ __device__ inline size_t group_smem_bytes(int W, int n_sm, size_t stride, size_t xs, int levels, int ntab) {
   return (smem_layout(W, n_sm, stride, xs, levels, ntab).total + 127) & ~(size_t)127;   // the CTA-shared area behind the groups stays 128-byte aligned
 }
 
-template <int EPL, int FAM, int W, bool DN, int G, bool MM, bool DP>
-__device__ __forceinline__ void setup_backend(DeviceBackend<EPL, FAM, W, DN, G, MM, DP>& b, const KArgs& a,
+template <int EPL, int FAM, int W, bool DN, int G, bool DP>
+__device__ __forceinline__ void setup_backend(DeviceBackend<EPL, FAM, W, DN, G, DP>& b, const KArgs& a,
                                               unsigned char* smem) {
   b.ctid = threadIdx.x; b.grp = 0;
   b.tid = threadIdx.x; b.lane = threadIdx.x & 31; b.warp = threadIdx.x >> 5;
@@ -97,43 +87,28 @@ __device__ __forceinline__ void setup_backend(DeviceBackend<EPL, FAM, W, DN, G, 
   const SmemLayout L = smem_layout(W, a.n_sm, b.stride, (size_t)a.xs_doubles, DP ? a.levels : kStdLevels, DP ? a.ntab : kStdTab);
   b.lX = a.lX; b.lXt = a.lXt; b.ly = a.ly; b.lN = a.lN; b.lLd = a.lLd;
   b.lr = a.lr ? a.lr + (size_t)blockIdx.x * a.lN : nullptr;
-  b.lll = nullptr; b.cb_flags = nullptr; b.cb_beta = b.cb_grad = b.cb_stage = nullptr;
+  b.cb_beta = b.cb_grad = nullptr;
   b.cb_shared = nullptr; b.ring_n = 0; b.lXp = nullptr; b.Mp = a.minv_pad; b.pooled = a.pooled;
-  b.prof = a.prof ? a.prof + (size_t)blockIdx.x * 32 * 16 : nullptr;
   size_t group = blockIdx.x;
-  if constexpr (G > 1) {
-    b.grp = threadIdx.x / (32 * W); b.tid = threadIdx.x % (32 * W); b.warp = b.tid >> 5;
+  if constexpr (G > 1) {                               // one warp per chain
+    b.grp = threadIdx.x >> 5; b.tid = threadIdx.x & 31; b.warp = 0;
     group = (size_t)blockIdx.x * G + b.grp;
     const size_t per = group_smem_bytes(W, a.n_sm, b.stride, (size_t)a.xs_doubles, DP ? a.levels : kStdLevels, DP ? a.ntab : kStdTab);
     unsigned char* shared = smem + per * G;            // the area after the G per-group blocks (128-byte aligned)
     b.cb_shared = shared;
-    b.cb_flags = reinterpret_cast<int*>(shared);
-    if constexpr (MM) {
-      b.cb_beta = reinterpret_cast<double*>(shared + tma_beta_off());
-      b.cb_stage = reinterpret_cast<double*>(shared + tma_ring_off(G));
-      b.cb_grad = b.cb_stage;                          // Xᵀr [chain][XS] is handed back in stage 0 of the idle ring
-      const int nzero = (int)((tma_tabs_off(G) - tma_beta_off()) / sizeof(double));    // β (incl. its zero k-padding), η, residual tiles
-      for (int i = threadIdx.x; i < nzero; i += 32 * W * G) b.cb_beta[i] = 0.0;
-      double* tabs = reinterpret_cast<double*>(shared + tma_tabs_off(G));
-      for (int i = threadIdx.x; i < DM_TABS_DOUBLES; i += 32 * W * G) tabs[i] = dm_tabs_entry(i);
-      if (threadIdx.x == 0) {
-        uint64_t* bars = reinterpret_cast<uint64_t*>(shared + 64);
-        for (int s = 0; s < kTmaStages; ++s) { mbar_init(bars + s, 1); mbar_init(bars + kTmaStages + s, W * G); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-      }
-      b.lXp = a.lXp;
-      b.lr = nullptr;
-      b.lll = a.lr + (size_t)blockIdx.x * G * a.lN;         // ll terms [G][N]
-    } else {
-      b.cb_beta = reinterpret_cast<double*>(shared + 64);
-      b.cb_stage = b.cb_beta + coop_beta_doubles(G);
-      b.cb_grad = b.cb_stage;
-      static_assert(coop_stage_doubles(G) >= 32 * G * G, "Xᵀr fits in one stage");
-      for (int i = threadIdx.x; i < (int)coop_beta_doubles(G); i += 32 * W * G) b.cb_beta[i] = 0.0;
-      for (int i = threadIdx.x; i < (int)coop_ring_doubles(G); i += 32 * W * G) b.cb_stage[i] = 0.0;
-      b.lr = a.lr + (size_t)blockIdx.x * 2 * G * a.lN;       // residuals [N][G]
-      b.lll = b.lr + (size_t)G * a.lN;                       // ll terms   [G][N]
+    b.cb_beta = reinterpret_cast<double*>(shared + tma_beta_off());
+    b.cb_grad = reinterpret_cast<double*>(shared + tma_ring_off(G));   // Xᵀr [chain][XS] is handed back in stage 0 of the idle ring
+    const int nzero = (int)((tma_tabs_off(G) - tma_beta_off()) / sizeof(double));    // β (incl. its zero k-padding), η, residual tiles
+    for (int i = threadIdx.x; i < nzero; i += 32 * G) b.cb_beta[i] = 0.0;
+    double* tabs = reinterpret_cast<double*>(shared + tma_tabs_off(G));
+    for (int i = threadIdx.x; i < DM_TABS_DOUBLES; i += 32 * G) tabs[i] = dm_tabs_entry(i);
+    if (threadIdx.x == 0) {
+      uint64_t* bars = reinterpret_cast<uint64_t*>(shared + 64);
+      for (int s = 0; s < kTmaStages; ++s) { mbar_init(bars + s, 1); mbar_init(bars + kTmaStages + s, G); }
+      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
+    b.lXp = a.lXp;
+    b.lr = nullptr;
     smem += per * b.grp;
     __syncthreads();
   }
@@ -152,19 +127,12 @@ __device__ __forceinline__ void setup_backend(DeviceBackend<EPL, FAM, W, DN, G, 
   b.mparams = a.mparams;
 }
 
-// packed groups: every chain group draws its own chains
+// packed groups: every warp draws its own chains
 template <class B>
-__device__ __forceinline__ int next_chain_group(B& b, unsigned* counter, int* s_misc, int begin) {
-  if constexpr (B::W == 1) {
-    int c = 0;
-    if (b.lane == 0) c = begin + (int)atomicAdd(counter, 1u);
-    return __shfl_sync(0xffffffffu, c, 0);
-  } else {
-    b.group_sync();
-    if (b.tid == 0) s_misc[0] = begin + (int)atomicAdd(counter, 1u);
-    b.group_sync();
-    return s_misc[0];
-  }
+__device__ __forceinline__ int next_chain_group(B& b, unsigned* counter, int begin) {
+  int c = 0;
+  if (b.lane == 0) c = begin + (int)atomicAdd(counter, 1u);
+  return __shfl_sync(0xffffffffu, c, 0);
 }
 // pooled metric: the whole CTA (8 chains = one metric group) takes group g; warp w runs chain begin + 8·g + w.  All warps
 // arrive here together (they left the previous group through coop_finish), so a CTA barrier is safe.
@@ -183,8 +151,8 @@ __device__ __forceinline__ int next_chain(unsigned* counter, int* s_misc, int be
   return s_misc[0];
 }
 
-template <int EPL, int FAM, int W, bool DN, int G, bool MM, bool DP>
-__device__ __forceinline__ void load_chain(DeviceBackend<EPL, FAM, W, DN, G, MM, DP>& b, const KArgs& a, long c,
+template <int EPL, int FAM, int W, bool DN, int G, bool DP>
+__device__ __forceinline__ void load_chain(DeviceBackend<EPL, FAM, W, DN, G, DP>& b, const KArgs& a, long c,
                                            bool with_p) {
   b.chain = c;
   b.rexp_base = 0xffffffffu; b.rexp_t = 0xffffffffu;   // the randexp batch belongs to one chain
@@ -209,8 +177,8 @@ __device__ __forceinline__ void load_chain(DeviceBackend<EPL, FAM, W, DN, G, MM,
     if (with_p) b.matvec(b.p, b.ps);
   }
 }
-template <int EPL, int FAM, int W, bool DN, int G, bool MM, bool DP>
-__device__ __forceinline__ void store_vec(const DeviceBackend<EPL, FAM, W, DN, G, MM, DP>& b, double* dst,
+template <int EPL, int FAM, int W, bool DN, int G, bool DP>
+__device__ __forceinline__ void store_vec(const DeviceBackend<EPL, FAM, W, DN, G, DP>& b, double* dst,
                                           const double (&v)[EPL], size_t base, int D) {
 #pragma unroll
   for (int e = 0; e < EPL; ++e) {
@@ -220,9 +188,9 @@ __device__ __forceinline__ void store_vec(const DeviceBackend<EPL, FAM, W, DN, G
 }
 
 // ------------------------------------------------------------------ k_nuts
-template <int EPL, int FAM, int W, bool DN, int G, bool MM, bool DP>
+template <int EPL, int FAM, int W, bool DN, int G, bool DP>
 struct DrawSink {
-  DeviceBackend<EPL, FAM, W, DN, G, MM, DP>& b;
+  DeviceBackend<EPL, FAM, W, DN, G, DP>& b;
   const KArgs& a;
   long c;
   __device__ __forceinline__ void operator()(int n, const dhmc_tree_stats& ts, double e) {
@@ -246,29 +214,26 @@ struct DrawSink {
   }
 };
 
-template <int EPL, int FAM, int W, bool DN, int G = 1, bool MM = false, bool DP = false>
+template <int EPL, int FAM, int W, bool DN, int G = 1, bool DP = false>
 __global__ void __launch_bounds__(32 * W * G, G > 1 ? 1 : min_ctas(W, EPL)) k_nuts(const KArgs a) {
   extern __shared__ __align__(128) unsigned char smem[];
-  DeviceBackend<EPL, FAM, W, DN, G, MM, DP> b;
-#ifdef DHMC_PROFILE_ROUNDS
-  const long long pf_kernel_t0 = clock64();
-#endif
+  DeviceBackend<EPL, FAM, W, DN, G, DP> b;
   setup_backend(b, a, smem);
-  int* s_misc = reinterpret_cast<int*>(smem + (G > 1 ? b.grp * group_smem_bytes(W, a.n_sm, b.stride, (size_t)a.xs_doubles, DP ? a.levels : kStdLevels, DP ? a.ntab : kStdTab) : 0) +
-                                       smem_layout(W, a.n_sm, b.stride, (size_t)a.xs_doubles, DP ? a.levels : kStdLevels, DP ? a.ntab : kStdTab).misc_off);
+  int* s_misc = reinterpret_cast<int*>(smem + smem_layout(W, a.n_sm, b.stride, (size_t)a.xs_doubles, DP ? a.levels : kStdLevels,
+                                                          DP ? a.ntab : kStdTab).misc_off);   // one chain per CTA: the queue's broadcast slot
   for (;;) {
     int c;
     if constexpr (G > 1) {
-      if (MM && a.pooled) c = next_pooled_group(b, a.counter, a.chain_begin);    // the CTA takes a whole metric group
-      else c = next_chain_group(b, a.counter, s_misc, a.chain_begin);
+      if (a.pooled) c = next_pooled_group(b, a.counter, a.chain_begin);    // the CTA takes a whole metric group
+      else c = next_chain_group(b, a.counter, a.chain_begin);
     } else {
       c = next_chain(a.counter, s_misc, a.chain_begin);
     }
     if (c >= a.chain_end) break;
     load_chain(b, a, c, false);
-    NutsMachine<DeviceBackend<EPL, FAM, W, DN, G, MM, DP>> m(b, dm_make_key(a.seed, (uint64_t)(a.chain_offset + c)),
+    NutsMachine<DeviceBackend<EPL, FAM, W, DN, G, DP>> m(b, dm_make_key(a.seed, (uint64_t)(a.chain_offset + c)),
                                            a.max_depth, a.min_delta, a.n_slots);
-    DrawSink<EPL, FAM, W, DN, G, MM, DP> sink{b, a, c};
+    DrawSink<EPL, FAM, W, DN, G, DP> sink{b, a, c};
     const double eps_next = m.run(a.t0, a.N, a.eps[c], a.cfg, a.p_override,
                                   a.dir_override ? a.dir_override + c : nullptr, sink);
     const size_t base = (size_t)c * a.D;
@@ -281,40 +246,37 @@ __global__ void __launch_bounds__(32 * W * G, G > 1 ? 1 : min_ctas(W, EPL)) k_nu
       if (m.status) atomicOr(a.status + c, m.status);
       atomicAdd(a.total_steps, (unsigned long long)m.steps_out);
     }
-    if constexpr (G > 1 && MM) { if (a.pooled) b.coop_finish(); }     // pooled metric: the group leaves together, then the CTA takes the next one
+    if constexpr (G > 1) { if (a.pooled) b.coop_finish(); }     // pooled metric: the group leaves together, then the CTA takes the next one
   }
   b.coop_finish();
-#ifdef DHMC_PROFILE_ROUNDS
-  if (b.prof && b.lane == 0) b.prof[(size_t)(threadIdx.x >> 5) * 16 + 9] += (unsigned long long)(clock64() - pf_kernel_t0);
-#endif
 }
 
 // ------------------------------------------------------------------ k_search
-template <int EPL, int FAM, int W, bool DN, int G = 1, bool MM = false, bool DP = false>
+template <int EPL, int FAM, int W, bool DN, int G = 1, bool DP = false>
 __global__ void __launch_bounds__(32 * W * G, G > 1 ? 1 : min_ctas(W, EPL)) k_search(const KArgs a) {
   extern __shared__ __align__(128) unsigned char smem[];
-  DeviceBackend<EPL, FAM, W, DN, G, MM, DP> b;
+  DeviceBackend<EPL, FAM, W, DN, G, DP> b;
   setup_backend(b, a, smem);
-  int* s_misc = reinterpret_cast<int*>(smem + (G > 1 ? b.grp * group_smem_bytes(W, a.n_sm, b.stride, (size_t)a.xs_doubles, DP ? a.levels : kStdLevels, DP ? a.ntab : kStdTab) : 0) +
-                                       smem_layout(W, a.n_sm, b.stride, (size_t)a.xs_doubles, DP ? a.levels : kStdLevels, DP ? a.ntab : kStdTab).misc_off);
+  int* s_misc = reinterpret_cast<int*>(smem + smem_layout(W, a.n_sm, b.stride, (size_t)a.xs_doubles, DP ? a.levels : kStdLevels,
+                                                          DP ? a.ntab : kStdTab).misc_off);   // one chain per CTA: the queue's broadcast slot
   for (;;) {
     int c;
     if constexpr (G > 1) {
-      if (MM && a.pooled) c = next_pooled_group(b, a.counter, a.chain_begin);
-      else c = next_chain_group(b, a.counter, s_misc, a.chain_begin);
+      if (a.pooled) c = next_pooled_group(b, a.counter, a.chain_begin);
+      else c = next_chain_group(b, a.counter, a.chain_begin);
     } else {
       c = next_chain(a.counter, s_misc, a.chain_begin);
     }
     if (c >= a.chain_end) break;
     load_chain(b, a, c, false);
-    NutsMachine<DeviceBackend<EPL, FAM, W, DN, G, MM, DP>> m(b, dm_make_key(a.seed, (uint64_t)(a.chain_offset + c)),
+    NutsMachine<DeviceBackend<EPL, FAM, W, DN, G, DP>> m(b, dm_make_key(a.seed, (uint64_t)(a.chain_offset + c)),
                                            a.max_depth, a.min_delta, a.n_slots);
     const double eps = m.find_initial_stepsize(a.s_init, a.s_thresh, a.s_maxiter, a.p_override);
     if (b.tid == 0) {
       a.eps[c] = eps;
       if (m.status) atomicOr(a.status + c, m.status);
     }
-    if constexpr (G > 1 && MM) { if (a.pooled) b.coop_finish(); }
+    if constexpr (G > 1) { if (a.pooled) b.coop_finish(); }
   }
   b.coop_finish();
 }
@@ -405,30 +367,29 @@ inline bool layout_supported(int W, int epl) {
 // dense (Symmetric metric) kernels are instantiated for every layout (D <= 2048; memory: 3·D² doubles per chain)
 constexpr bool dense_layout(int W, int EPL) { return W >= 1 && EPL >= 1; }
 constexpr int kPack = 8;            // packed chain groups: chains per CTA (logistic family, dim <= 256)
-// packed layouts for dim <= 256: one warp per chain (up to 8 elements per lane) or two (dim 129…256)
-constexpr bool packed_layout(int W, int EPL) { return (W == 1) || (W == 2 && EPL == 4); }
+// packed layouts for dim <= 256: one warp per chain, up to 8 elements per lane
+constexpr bool packed_layout(int W, int EPL) { return W == 1; }
 
 // which subset of a family's kernels a translation unit instantiates (build parallelism):
-//   PART 0: one chain per CTA;  PART 1: packed groups, FMA likelihood;  PART 2: packed groups, tensor-core likelihood;
+//   PART 0: one chain per CTA;  PART 1: packed groups, tensor-core likelihood;
 //   PART 3: one chain per CTA, max_depth > 12 (k_nuts / k_search only)
 template <int EPL, int FAM, int W, int PART>
 const void* kernel_ptr(KernelId k, bool dense) {
   if constexpr (PART == 3) {        // max_depth > 12: one chain per CTA, slot pool with spill words
     if (dense) {
       if constexpr (dense_layout(W, EPL)) {
-        if (k == K_NUTS) return (const void*)k_nuts<EPL, FAM, W, true, 1, false, true>;
-        if (k == K_SEARCH) return (const void*)k_search<EPL, FAM, W, true, 1, false, true>;
+        if (k == K_NUTS) return (const void*)k_nuts<EPL, FAM, W, true, 1, true>;
+        if (k == K_SEARCH) return (const void*)k_search<EPL, FAM, W, true, 1, true>;
       }
       return nullptr;
     }
-    if (k == K_NUTS) return (const void*)k_nuts<EPL, FAM, W, false, 1, false, true>;
-    if (k == K_SEARCH) return (const void*)k_search<EPL, FAM, W, false, 1, false, true>;
+    if (k == K_NUTS) return (const void*)k_nuts<EPL, FAM, W, false, 1, true>;
+    if (k == K_SEARCH) return (const void*)k_search<EPL, FAM, W, false, 1, true>;
     return nullptr;
-  } else if constexpr (PART > 0) {
+  } else if constexpr (PART == 1) {
     if constexpr (FAM == DHMC_FAMILY_LOGISTIC && packed_layout(W, EPL)) {
-      constexpr bool MM = PART == 2;
-      if (k == K_NUTS) return dense ? (const void*)k_nuts<EPL, FAM, W, true, kPack, MM> : (const void*)k_nuts<EPL, FAM, W, false, kPack, MM>;
-      if (k == K_SEARCH) return dense ? (const void*)k_search<EPL, FAM, W, true, kPack, MM> : (const void*)k_search<EPL, FAM, W, false, kPack, MM>;
+      if (k == K_NUTS) return dense ? (const void*)k_nuts<EPL, FAM, W, true, kPack> : (const void*)k_nuts<EPL, FAM, W, false, kPack>;
+      if (k == K_SEARCH) return dense ? (const void*)k_search<EPL, FAM, W, true, kPack> : (const void*)k_search<EPL, FAM, W, false, kPack>;
     }
     return nullptr;
   } else {
