@@ -18,7 +18,7 @@ tree_stats_dtype = np.dtype(
      ("acceptance_rate", "<f8"), ("steps", "<i8"), ("directions", "<u4"), ("pad", "<u4")])
 
 EXPORTS = [
-    "dhmc_create", "dhmc_destroy", "dhmc_last_error", "dhmc_get_layout", "dhmc_set_problem", "dhmc_user_family_name",
+    "dhmc_create", "dhmc_destroy", "dhmc_last_error", "dhmc_get_layout", "dhmc_set_problem", "dhmc_set_problems", "dhmc_user_family_name",
     "dhmc_family_available",
     "dhmc_set_position", "dhmc_random_position", "dhmc_set_metric", "dhmc_set_metric_dense",
     "dhmc_get_metric_dense", "dhmc_metric_is_dense", "dhmc_set_stepsize",
@@ -26,7 +26,7 @@ EXPORTS = [
     "dhmc_set_transition_count", "dhmc_leapfrog", "dhmc_phase_logdensity", "dhmc_sample_tree",
     "dhmc_find_initial_stepsize", "dhmc_warmup_stage", "dhmc_mcmc", "dhmc_mcmc_from", "dhmc_mcmc_dev",
     "dhmc_tree_summary_dev", "dhmc_last_total_steps", "dhmc_last_kernel_ms", "dhmc_kernel_launches",
-    "dhmc_ess_rhat_dev", "dhmc_acceptance_quantiles_dev", "dhmc_mcmc_thinned", "dhmc_host_alloc", "dhmc_host_free",
+    "dhmc_ess_rhat_dev", "dhmc_ess_rhat_problems_dev", "dhmc_acceptance_quantiles_dev", "dhmc_mcmc_thinned", "dhmc_host_alloc", "dhmc_host_free",
     "dhmc_comm_unique_id", "dhmc_comm_init", "dhmc_comm_destroy", "dhmc_allgather_dev",
     "dhmc_allgather_positions_dev", "dhmc_last_comm_ms",
 ]

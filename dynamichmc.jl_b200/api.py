@@ -234,6 +234,66 @@ class UserLogDensity(DeviceLogDensity):
         return self._cpu(np.asarray(q, float))
 
 
+# ------------------------------------------------------------------ problem batches
+class ProblemBatch:
+    """Many posteriors on one handle (dhmc_set_problems): `problems` are P log densities of one family and dimension whose
+    parameter blocks have equal length (logistic regression: the same N), each sampled by `chains_per_problem` chains.
+    Global chain g samples problem g // chains_per_problem, and those chains are bit-identical to a handle that holds
+    problem p alone with chain_offset = p·chains_per_problem — for simulation-based calibration, bootstrap or
+    cross-validation refits and one fit per unit, which need many posteriors and only a few chains each.  Validated on
+    the host; hand it to Engine / mcmc_with_warmup in place of ℓ."""
+
+    def __init__(self, problems, chains_per_problem):
+        problems = list(problems)
+        _argcheck(len(problems) >= 1, "a batch needs at least one problem")
+        _argcheck(all(isinstance(x, DeviceLogDensity) for x in problems), "problems: DeviceLogDensity objects")
+        self.chains_per_problem = int(chains_per_problem)
+        _argcheck(self.chains_per_problem >= 1, "chains_per_problem ≥ 1")
+        first = problems[0]
+        self.family, self.D = first.family, int(first.dimension())
+        _argcheck(all(x.family == self.family for x in problems), "every problem of a batch has the same family")
+        _argcheck(all(int(x.dimension()) == self.D for x in problems), "every problem of a batch has the same dimension")
+        _argcheck(self.family not in (L.FAMILY_STD_NORMAL, L.FAMILY_FUNNEL),
+                  "this family has no parameters: a batch of it would be one problem")
+        self.library_path = getattr(first, "library_path", None)
+        _argcheck(all(getattr(x, "library_path", None) == self.library_path for x in problems),
+                  "every problem of a batch lives in the same user-model library")
+        blocks = [np.ascontiguousarray(x.params(), float).ravel() for x in problems]
+        if self.family == L.FAMILY_LOGISTIC:
+            _argcheck(all(b[0] == blocks[0][0] for b in blocks), "every logistic problem of a batch has the same N")
+        _argcheck(all(b.size == blocks[0].size for b in blocks), "every problem of a batch has a parameter block of the same length")
+        _argcheck(blocks[0].size >= 1, "the problems have empty parameter blocks")
+        self.problems = problems
+        self.block_size = blocks[0].size
+        self._params = np.concatenate(blocks)
+
+    @property
+    def n_problems(self):
+        return len(self.problems)
+
+    @property
+    def chains(self):
+        """chains of the whole batch: n_problems · chains_per_problem"""
+        return self.n_problems * self.chains_per_problem
+
+    def dimension(self):
+        return self.D
+
+    def capabilities(self):
+        return min(x.capabilities() for x in self.problems)
+
+    def params(self):
+        """the P blocks back to back, [P · block_size]"""
+        return self._params
+
+    def problem_chains(self, p, chain_offset=0, chains=None):
+        """local chain range [lo, hi) of problem p on a handle with `chains` chains from global id `chain_offset`"""
+        chains = self.chains - chain_offset if chains is None else chains
+        K = self.chains_per_problem
+        lo, hi = max(p * K - chain_offset, 0), min((p + 1) * K - chain_offset, chains)
+        return lo, max(lo, hi)
+
+
 # ------------------------------------------------------------------ algorithm structs
 @dataclass
 class NUTS:
@@ -331,7 +391,7 @@ class GaussianKineticEnergy:
 
 # ------------------------------------------------------------------ engine
 class Engine:
-    """Owns a dhmc_handle: K chains of one problem on one GPU."""
+    """Owns a dhmc_handle: K chains of one problem (or of a ProblemBatch) on one GPU."""
 
     def __init__(self, ℓ: DeviceLogDensity, chains: int, seed: int = 0, algorithm: NUTS = None,
                  device: int = 0, chain_offset: int = 0, threads_per_chain: int = 0,
@@ -352,8 +412,21 @@ class Engine:
                 raise ArgumentError(msg)
             raise RuntimeError(f"dhmc_create failed [{rc}]: {msg}")
         self._h = h
+        self._set_problem(ℓ)
+
+    def _set_problem(self, ℓ):
+        """dhmc_set_problem, or dhmc_set_problems for a ProblemBatch.  On an error the handle keeps its previous problem."""
+        if self.ℓ is not ℓ:                              # replacing the problem of an existing handle
+            _argcheck(ℓ.family == self.ℓ.family and int(ℓ.dimension()) == self.D, "same family and dimension as the handle")
+            _argcheck(getattr(ℓ, "library_path", None) == getattr(self.ℓ, "library_path", None),
+                      "a user model of the handle's own library")
         pr = np.ascontiguousarray(ℓ.params(), float)
-        self._ck(self._lib.dhmc_set_problem(self._h, L.ptr(pr) if pr.size else None, C.c_size_t(pr.size)))
+        if isinstance(ℓ, ProblemBatch):
+            self._ck(self._lib.dhmc_set_problems(self._h, L.ptr(pr), C.c_size_t(ℓ.block_size), C.c_int64(ℓ.n_problems),
+                                                 C.c_int64(ℓ.chains_per_problem)))
+        else:
+            self._ck(self._lib.dhmc_set_problem(self._h, L.ptr(pr) if pr.size else None, C.c_size_t(pr.size)))
+        self.ℓ = ℓ
 
     # -- plumbing
     def _ck(self, rc):
@@ -649,6 +722,16 @@ class Engine:
                                              L.ptr(rhat), L.ptr(ess)))
         return dict(rhat=rhat, ess=ess)
 
+    def ess_rhat_problems_dev(self, draws_ptr, N, max_lag=0):
+        """split-R̂ and ESS per (problem, parameter) of a ProblemBatch, each over its problem's local chains, from a DEVICE
+        draws buffer [K, N, D] (dhmc_ess_rhat_problems_dev) → rhat, ess [P, D]; NaN for a problem without local chains."""
+        _argcheck(isinstance(self.ℓ, ProblemBatch), "the engine holds no ProblemBatch")
+        P = self.ℓ.n_problems
+        rhat, ess = np.empty((P, self.D)), np.empty((P, self.D))
+        self._ck(self._lib.dhmc_ess_rhat_problems_dev(self._h, C.c_void_p(draws_ptr), C.c_int32(N), C.c_int32(max_lag),
+                                                      L.ptr(rhat), L.ptr(ess)))
+        return dict(rhat=rhat, ess=ess)
+
     def acceptance_quantiles_dev(self, stats_ptr, N, probs=(0.05, 0.25, 0.5, 0.75, 0.95)):
         """a_quantiles of summarize_tree_statistics (diagnostics.jl:35) from a DEVICE statistics buffer."""
         pr = np.ascontiguousarray(probs, float)
@@ -691,6 +774,18 @@ class Results(Sequence):
                 "tree_statistics": self._stats[k], "logdensities": self._logd[k],
                 "κ": GaussianKineticEnergy(self._minv[k], dense=self._minv[k].ndim == 2), "ϵ": float(self._eps[k]),
                 "eps": float(self._eps[k])}
+
+
+def results_by_problem(results: Results, batch: ProblemBatch, chain_offset=0):
+    """The Results of a ProblemBatch run split per problem: element p holds problem p's local chains (zero-copy views;
+    empty for a problem with no chain on this handle).  `chain_offset` is the handle's (a shard of the batch)."""
+    B = len(results)
+    out = []
+    for p in range(batch.n_problems):
+        lo, hi = batch.problem_chains(p, chain_offset, B)
+        out.append(Results(results._post[lo:hi], results._stats[lo:hi], results._logd[lo:hi], results._minv[lo:hi],
+                           results._eps[lo:hi]))
+    return out
 
 
 def stack_posterior_matrices(results: Results):
@@ -737,9 +832,17 @@ def _report(reporter, message, **kw):
         pass
 
 
-def mcmc_keep_warmup(seed, ℓ, N, chains=1, initialization=None, warmup_stages=None,
+def _default_chains(ℓ, chains, chain_offset):
+    if chains is not None:
+        return chains
+    return ℓ.chains - chain_offset if isinstance(ℓ, ProblemBatch) else 1
+
+
+def mcmc_keep_warmup(seed, ℓ, N, chains=None, initialization=None, warmup_stages=None,
                      algorithm=None, keep_warmup=True, device=0, chain_offset=0, engine_opts=None, reporter=None):
-    """src/mcmc.jl:521-532 for `chains` chains at once."""
+    """src/mcmc.jl:521-532 for `chains` chains at once (default 1; for a ProblemBatch every chain of the batch from
+    chain_offset on)."""
+    chains = _default_chains(ℓ, chains, chain_offset)
     stages = default_warmup_stages() if warmup_stages is None else warmup_stages
     eng = Engine(ℓ, chains, seed=seed, algorithm=algorithm, device=device, chain_offset=chain_offset,
                  **(engine_opts or {}))
@@ -766,9 +869,9 @@ def mcmc_keep_warmup(seed, ℓ, N, chains=1, initialization=None, warmup_stages=
     return dict(warmup=warm, inference=results, engine=eng)
 
 
-def mcmc_with_warmup(seed, ℓ, N, chains=1, initialization=None, warmup_stages=None, algorithm=None,
+def mcmc_with_warmup(seed, ℓ, N, chains=None, initialization=None, warmup_stages=None, algorithm=None,
                      device=0, chain_offset=0, engine_opts=None, reporter=None):
-    """src/mcmc.jl:575-584 for `chains` chains at once → Results."""
+    """src/mcmc.jl:575-584 for `chains` chains at once → Results (a ProblemBatch: results_by_problem splits them)."""
     r = mcmc_keep_warmup(seed, ℓ, N, chains=chains, initialization=initialization,
                          warmup_stages=warmup_stages, algorithm=algorithm, keep_warmup=False,
                          device=device, chain_offset=chain_offset, engine_opts=engine_opts, reporter=reporter)

@@ -248,17 +248,24 @@ __global__ void k_tree_summary(const dhmc_tree_stats* stats, int N, int B, unsig
 // ---- cross-chain convergence diagnostics on device-resident draws [B][N][D] (§8f-2; the reference's tests use
 // MCMCDiagnosticTools.ess_rhat on the same quantities, sample-correctness_utilities.jl:40-43).  Every chain is split in
 // two halves of n = N/2 draws (m = 2B sequences).  One warp = 32 consecutive parameters of one sequence: mean, then the
-// biased autocovariances at lags 0…L; the per-parameter sums over sequences are accumulated with atomics:
-//   acc[d][0] = Σ (μ − pilot_d), [1] = Σ (μ − pilot_d)², [2 + t] = Σ acov(t)        (pilot_d = mean of sequence 0: a shift
-//   that keeps the variance of the means free of cancellation).  The host finishes R̂ and the Geyer sum (tiny).
-__global__ void k_pilot_mean(const double* draws, int n, int N, int D, double* pilot) {
-  const int d = blockIdx.x * blockDim.x + threadIdx.x;
-  if (d >= D) return;
+// biased autocovariances at lags 0…L; the per-parameter sums over the sequences of a chain group are accumulated with atomics:
+//   acc[g][d][0] = Σ (μ − pilot_gd), [1] = Σ (μ − pilot_gd)², [2 + t] = Σ acov(t)   (pilot_gd = mean of the group's first
+//   sequence: a shift that keeps the variance of the means free of cancellation).  The host finishes R̂ and the Geyer sum.
+// Chain groups: local chain c belongs to group (off + c) / K — the problems of a batch; K = 0: one group of all chains.
+__device__ __forceinline__ int ess_group(long c, long long K, long long off) { return K ? (int)((off + c) / K) : 0; }
+__global__ void k_pilot_mean(const double* draws, int n, int N, int D, int B, long long K, long long off, int P, double* pilot) {
+  const long t = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= (long)P * D) return;
+  const int g = (int)(t / D), d = (int)(t % D);
+  const long long first = (long long)g * K - off;
+  const long c0 = (K && first > 0) ? (long)first : 0;                            // the group's first local chain
+  if (c0 >= B || ess_group(c0, K, off) != g) return;                            // no local chain: the host reports NaN
   double s = 0.0;
-  for (int i = 0; i < n; ++i) s += draws[(size_t)i * D + d];
-  pilot[d] = s / n;
+  for (int i = 0; i < n; ++i) s += draws[((size_t)c0 * N + i) * D + d];
+  pilot[t] = s / n;
 }
-__global__ void k_ess_rhat(const double* draws, int N, int n, int D, int B, int L, const double* pilot, double* acc) {
+__global__ void k_ess_rhat(const double* draws, int N, int n, int D, int B, long long K, long long off, int L, const double* pilot,
+                           double* acc) {
   const int lane = threadIdx.x & 31;
   const long warp = ((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = ((long)gridDim.x * blockDim.x) >> 5;
   const int tiles = (D + 31) / 32;
@@ -271,8 +278,9 @@ __global__ void k_ess_rhat(const double* draws, int N, int n, int D, int B, int 
     double mu = 0.0;
     for (int i = 0; i < n; ++i) mu += x[(size_t)i * D];
     mu /= n;
-    double* a = acc + (size_t)d * (L + 3);
-    const double dm = mu - pilot[d];
+    const size_t gd = (size_t)ess_group(seq >> 1, K, off) * D + d;
+    double* a = acc + gd * (L + 3);
+    const double dm = mu - pilot[gd];
     atomicAdd(a, dm);
     atomicAdd(a + 1, dm * dm);
     for (int t = 0; t <= L; ++t) {
@@ -346,6 +354,10 @@ struct dhmc_handle {
   double *lX = nullptr, *lXt = nullptr, *ly = nullptr, *lr = nullptr;   // logistic regression
   double* lXp = nullptr;            // … zero-padded row blocks of X for the tensor-core likelihood
   int lN = 0, lLd = 0;
+  // problem batch (dhmc_set_problems): chains per problem (0 = one problem), problems, per-problem strides of the parameter
+  // arrays in doubles (mparams, lX, lXt, ly, lXp)
+  int64_t batch_k = 0, batch_p = 0;
+  size_t s_mparams = 0, s_lX = 0, s_lXt = 0, s_ly = 0, s_lXp = 0;
   int reg_ctas[2] = {0, 0};         // occupancy of k_nuts (diag, dense)
   size_t smem_sm = 0, smem_cta_max = 0;
   ncclComm_t comm = nullptr;        // multi-GPU: one communicator per handle (dhmc_comm_init)
@@ -456,6 +468,8 @@ static KArgs base_args(dhmc_handle* h) {
   a.minv_dense = h->minv_dense; a.wt = h->wt; a.covt = nullptr; a.minv_pad = h->minv_pad; a.mean_out = nullptr; a.pooled = h->pooled ? 1 : 0;
   a.xs_doubles = needs_staging(h) ? (int)((size_t)h->T * h->EPL) : 0;
   a.lX = h->lX; a.lXt = h->lXt; a.ly = h->ly; a.lr = h->lr; a.lN = h->lN; a.lLd = h->lLd; a.lXp = h->lXp;
+  a.batch_k = (int)h->batch_k;
+  a.s_mparams = h->s_mparams; a.s_lX = h->s_lX; a.s_lXt = h->s_lXt; a.s_ly = h->s_ly; a.s_lXp = h->s_lXp;
   return a;
 }
 
@@ -680,6 +694,11 @@ int dhmc_user_family_name(char* name, size_t cap) {
   return DHMC_OK;
 }
 
+static void clear_batch(dhmc_handle* h) {
+  h->batch_k = h->batch_p = 0;
+  h->s_mparams = h->s_lX = h->s_lXt = h->s_ly = h->s_lXp = 0;
+}
+
 int dhmc_set_problem(dhmc_handle* h, const double* params, size_t n) {
   if (!h) return DHMC_EARG;
   CK(cudaSetDevice(h->cfg.device));
@@ -693,6 +712,7 @@ int dhmc_set_problem(dhmc_handle* h, const double* params, size_t n) {
       const double yv = params[1 + N * D + i];
       if (!(yv >= 0.0 && yv <= 1.0)) { h->err = "dhmc_set_problem: logistic regression needs 0 <= y <= 1"; return DHMC_EARG; }
     }
+    clear_batch(h);
     cudaFree(h->lX); cudaFree(h->lXt); cudaFree(h->ly); cudaFree(h->lr); cudaFree(h->lXp);
     h->lX = h->lXt = h->ly = h->lr = h->lXp = nullptr;
     const size_t ld = (N + 1) & ~(size_t)1;                 // even leading dimension: 16-byte aligned row segments
@@ -716,6 +736,7 @@ int dhmc_set_problem(dhmc_handle* h, const double* params, size_t n) {
   }
   if (h->cfg.family == DHMC_FAMILY_USER) {      // any number of doubles, interpreted by the user's formulas
     if (n && !params) { h->err = "dhmc_set_problem: null parameter block"; return DHMC_EARG; }
+    clear_batch(h);
     CK(cudaStreamSynchronize(h->stream));
     cudaFree(h->mparams); h->mparams = nullptr;
     CK(cudaMalloc(&h->mparams, sizeof(double) * std::max<size_t>(n, 1)));
@@ -725,8 +746,91 @@ int dhmc_set_problem(dhmc_handle* h, const double* params, size_t n) {
   }
   const size_t want = h->cfg.family == DHMC_FAMILY_DIAG_NORMAL ? 2 * D : 0;
   if (n != want || (want && !params)) { h->err = "dhmc_set_problem: wrong parameter count for this family"; return DHMC_EARG; }
+  clear_batch(h);                                // (mparams holds at least 2·D doubles, also after a batch)
   if (want) CK(cudaMemcpyAsync(h->mparams, params, sizeof(double) * want, cudaMemcpyHostToDevice, h->stream));
   CK(cudaStreamSynchronize(h->stream));
+  return DHMC_OK;
+}
+
+// P problems of the handle's family and dimension, each with its own parameter block; global chain g samples problem
+// g / chains_per_problem.  Everything is validated before anything is allocated, and the new arrays are complete before
+// they replace the current ones: on any error the previous problem (batch or not) stays in effect.
+int dhmc_set_problems(dhmc_handle* h, const double* params, size_t n, int64_t P, int64_t K) {
+  if (!h) return DHMC_EARG;
+  const int fam = h->cfg.family;
+  const size_t D = (size_t)h->cfg.dim;
+  const int64_t off = h->cfg.chain_offset, B = h->cfg.n_chains;
+  if (fam != DHMC_FAMILY_DIAG_NORMAL && fam != DHMC_FAMILY_LOGISTIC && fam != DHMC_FAMILY_USER) {
+    h->err = "dhmc_set_problems: this family has no parameters (a batch of it would be one problem)"; return DHMC_EARG;
+  }
+  if (P < 1 || K < 1 || !params || n < 1) { h->err = "dhmc_set_problems: n_problems >= 1, chains_per_problem >= 1 and a parameter block per problem"; return DHMC_EARG; }
+  if (P * K > INT32_MAX) { h->err = "dhmc_set_problems: n_problems * chains_per_problem < 2^31"; return DHMC_EARG; }
+  if (off < 0 || off + B > P * K) {
+    h->err = "dhmc_set_problems: the handle's chains [chain_offset, chain_offset + n_chains) lie beyond n_problems * chains_per_problem";
+    return DHMC_EARG;
+  }
+  if (h->G > 1 && (K % 8 != 0 || off % 8 != 0 || B % 8 != 0)) {
+    h->err = "dhmc_set_problems: packed chain groups (logistic, automatic layout, dim <= 256) run 8 chains of one problem per CTA: "
+             "chains_per_problem, chain_offset and n_chains must be multiples of 8 (threads_per_chain=32 runs one chain per CTA without this condition)";
+    return DHMC_EARG;
+  }
+  size_t N = 0, ld = 0, rows = 0, xs = 0;
+  if (fam == DHMC_FAMILY_DIAG_NORMAL && n != 2 * D) { h->err = "dhmc_set_problems: DIAG_NORMAL blocks are [mu(D), prec(D)]"; return DHMC_EARG; }
+  if (fam == DHMC_FAMILY_LOGISTIC) {
+    N = params[0] >= 1 ? (size_t)params[0] : 0;
+    if (N < 1 || n != 1 + N * D + N) { h->err = "dhmc_set_problems: logistic blocks are [N, X (N*D), y (N)]"; return DHMC_EARG; }
+    for (int64_t p = 0; p < P; ++p) {
+      const double* blk = params + (size_t)p * n;
+      if (blk[0] != params[0]) { h->err = "dhmc_set_problems: every logistic problem of a batch needs the same N"; return DHMC_EARG; }
+      for (size_t i = 0; i < N; ++i) {
+        const double yv = blk[1 + N * D + i];
+        if (!(yv >= 0.0 && yv <= 1.0)) { h->err = "dhmc_set_problems: logistic regression needs 0 <= y <= 1"; return DHMC_EARG; }
+      }
+    }
+    ld = (N + 1) & ~(size_t)1;
+    rows = (N + kTmaRows - 1) / kTmaRows * kTmaRows;
+    xs = (size_t)tma_xs((int)D);
+  }
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->stream));
+  double *mp = nullptr, *X = nullptr, *Xt = nullptr, *y = nullptr, *Xp = nullptr, *lr = nullptr;
+  auto drop = [&] { cudaFree(mp); cudaFree(X); cudaFree(Xt); cudaFree(y); cudaFree(Xp); cudaFree(lr); };
+#define CKB(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { h->err = std::string(#call) + ": " + cudaGetErrorString(e_); \
+    cudaStreamSynchronize(h->stream); drop(); return e_ == cudaErrorMemoryAllocation ? DHMC_ENOMEM : DHMC_ECUDA; } } while (0)
+  const size_t Pz = (size_t)P;
+  if (fam == DHMC_FAMILY_LOGISTIC) {
+    // per problem: X [N][D], Xᵀ [D][ld], y [N] and, for packed groups, the zero-padded row blocks [rows][xs]
+    CKB(cudaMalloc(&X, sizeof(double) * Pz * N * D));
+    CKB(cudaMalloc(&Xt, sizeof(double) * Pz * ld * D));
+    CKB(cudaMalloc(&y, sizeof(double) * Pz * N));
+    CKB(cudaMalloc(&lr, sizeof(double) * N * lr_rows(h)));
+    if (h->G > 1) CKB(cudaMalloc(&Xp, sizeof(double) * Pz * rows * xs));
+    for (size_t p = 0; p < Pz; ++p) {
+      const double* blk = params + p * n;
+      CKB(cudaMemcpyAsync(X + p * N * D, blk + 1, sizeof(double) * N * D, cudaMemcpyHostToDevice, h->stream));
+      CKB(cudaMemcpyAsync(y + p * N, blk + 1 + N * D, sizeof(double) * N, cudaMemcpyHostToDevice, h->stream));
+      k_transpose<<<1024, 256, 0, h->stream>>>(X + p * N * D, Xt + p * ld * D, N, D, ld);
+      if (Xp) k_pad_rows<<<1024, 256, 0, h->stream>>>(X + p * N * D, Xp + p * rows * xs, N, D, rows, xs);
+      h->launches += Xp ? 2 : 1;
+    }
+  } else {
+    CKB(cudaMalloc(&mp, sizeof(double) * Pz * n));
+    CKB(cudaMemcpyAsync(mp, params, sizeof(double) * Pz * n, cudaMemcpyHostToDevice, h->stream));
+  }
+  CKB(cudaGetLastError());
+  CKB(cudaStreamSynchronize(h->stream));
+#undef CKB
+  if (fam == DHMC_FAMILY_LOGISTIC) {
+    cudaFree(h->lX); cudaFree(h->lXt); cudaFree(h->ly); cudaFree(h->lr); cudaFree(h->lXp);
+    h->lX = X; h->lXt = Xt; h->ly = y; h->lr = lr; h->lXp = Xp;
+    h->lN = (int)N; h->lLd = (int)ld;
+    h->s_mparams = 0; h->s_lX = N * D; h->s_lXt = ld * D; h->s_ly = N; h->s_lXp = Xp ? rows * xs : 0;
+  } else {
+    cudaFree(h->mparams);
+    h->mparams = mp;
+    h->s_mparams = n; h->s_lX = h->s_lXt = h->s_ly = h->s_lXp = 0;
+  }
+  h->batch_k = K; h->batch_p = P;
   return DHMC_OK;
 }
 
@@ -1046,8 +1150,8 @@ static int run_nuts(dhmc_handle* h, int N, const AdaptConfig& cfg, double lambda
   if (const char* ev = std::getenv("DHMC_E2E_CHUNKS")) { const int v = std::atoi(ev); if (v >= 1 && v <= 16 && !outputs_on_device) nchunks = v; }
   CKR(cudaMemsetAsync(h->status, 0, sizeof(int) * B, h->stream));   // status words describe the current call
   for (int ci = 0; ci < nchunks; ++ci) {
-    // (a pooled metric keeps its groups of 8 chains inside one chunk)
-    const size_t unit = h->pooled ? 8 : 1;
+    // (a pooled metric, and a batch on packed groups, keep their groups of 8 chains inside one chunk)
+    const size_t unit = (h->pooled || (h->G > 1 && h->batch_k)) ? 8 : 1;
     const size_t c0 = (B / unit) * ci / nchunks * unit, c1 = (B / unit) * (ci + 1) / nchunks * unit, nc = c1 - c0;
     if (nc == 0) continue;
     a.chain_begin = (int)c0; a.chain_end = (int)c1;
@@ -1151,6 +1255,7 @@ int dhmc_warmup_stage(dhmc_handle* h, int32_t N, int32_t metric, const dhmc_dual
       metric != DHMC_METRIC_SYMMETRIC_POOLED) { h->err = "metric: Nothing, Diagonal, Symmetric (or the pooled Symmetric option)"; return DHMC_EARG; }
   const bool pool = metric == DHMC_METRIC_SYMMETRIC_POOLED;
   if (pool && (h->cfg.n_chains % 8 != 0 || h->cfg.chain_offset % 8 != 0)) { h->err = "pooled metric: n_chains and chain_offset must be multiples of 8"; return DHMC_EARG; }
+  if (pool && h->batch_k % 8 != 0) { h->err = "pooled metric with a problem batch: chains_per_problem must be a multiple of 8 (a metric group never straddles two problems)"; return DHMC_EARG; }
   AdaptConfig cfg{};
   cfg.metric = pool ? DHMC_METRIC_SYMMETRIC : metric;
   if (da) {
@@ -1266,49 +1371,69 @@ int dhmc_tree_summary_dev(dhmc_handle* h, const dhmc_tree_stats* stats_dev, int3
   return DHMC_OK;
 }
 
-int dhmc_ess_rhat_dev(dhmc_handle* h, const double* draws_dev, int32_t N, int32_t max_lag, double* rhat, double* ess) {
-  if (!h || !draws_dev || N < 4 || (!rhat && !ess)) return DHMC_EARG;
+// split-R̂ and ESS of every (group, parameter): groups of K chains by global id (K = 0: all local chains form one group),
+// outputs rhat / ess [D, P] column-major; a group without local chains gets NaN.
+static int ess_rhat_groups(dhmc_handle* h, const double* draws_dev, int32_t N, int32_t max_lag, int64_t K, int P, double* rhat,
+                           double* ess) {
   CK(cudaSetDevice(h->cfg.device));
   const int D = (int)h->cfg.dim, B = (int)h->cfg.n_chains, n = N / 2;
+  const int64_t off = K ? h->cfg.chain_offset : 0;
   int L = max_lag > 0 ? max_lag : 64;
   if (L > n - 2) L = n - 2;
   if (L < 1) L = 1;
+  const size_t PD = (size_t)P * D;
   double *d_pilot = nullptr, *d_acc = nullptr;
-  CK(cudaMalloc(&d_pilot, sizeof(double) * D));
-  CK(cudaMalloc(&d_acc, sizeof(double) * (size_t)D * (L + 3)));
-  CK(cudaMemsetAsync(d_acc, 0, sizeof(double) * (size_t)D * (L + 3), h->stream));
-  k_pilot_mean<<<(D + 127) / 128, 128, 0, h->stream>>>(draws_dev, n, N, D, d_pilot);
-  k_ess_rhat<<<h->sm_count * 8, 256, 0, h->stream>>>(draws_dev, N, n, D, B, L, d_pilot, d_acc);
+  CK(cudaMalloc(&d_pilot, sizeof(double) * PD));
+  CK(cudaMalloc(&d_acc, sizeof(double) * PD * (L + 3)));
+  CK(cudaMemsetAsync(d_acc, 0, sizeof(double) * PD * (L + 3), h->stream));
+  k_pilot_mean<<<(unsigned)((PD + 127) / 128), 128, 0, h->stream>>>(draws_dev, n, N, D, B, K, off, P, d_pilot);
+  k_ess_rhat<<<h->sm_count * 8, 256, 0, h->stream>>>(draws_dev, N, n, D, B, K, off, L, d_pilot, d_acc);
   h->launches += 2;
-  std::vector<double> acc((size_t)D * (L + 3));
+  std::vector<double> acc(PD * (L + 3));
   cudaError_t e = cudaMemcpyAsync(acc.data(), d_acc, sizeof(double) * acc.size(), cudaMemcpyDeviceToHost, h->stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
   cudaFree(d_pilot); cudaFree(d_acc);
   if (e != cudaSuccess) { h->err = cudaGetErrorString(e); return DHMC_ECUDA; }
-  const double m = 2.0 * B, dn = (double)n;
-  for (int d = 0; d < D; ++d) {
-    const double* a = &acc[(size_t)d * (L + 3)];
-    const double mean_var = a[2] / m * dn / (dn - 1.0);                    // W: mean within-sequence variance (n − 1)
-    const double var_means = m > 1 ? (a[1] - a[0] * a[0] / m) / (m - 1.0) : 0.0;
-    const double var_plus = mean_var * (dn - 1.0) / dn + var_means;        // (n−1)/n·W + B/n
-    if (rhat) rhat[d] = std::sqrt(var_plus / mean_var);
-    if (ess) {
-      // Geyer's initial monotone sequence on ρ̂_t = 1 − (W − mean acov_t) / var⁺, pairs (ρ̂_2k + ρ̂_2k+1)
-      double tau = 0.0, prev = 1e300;
-      for (int t = 0; t + 1 <= L; t += 2) {
-        const double r0 = 1.0 - (mean_var - a[2 + t] / m) / var_plus, r1 = 1.0 - (mean_var - a[3 + t] / m) / var_plus;
-        double pair = r0 + r1;
-        if (!(pair > 0.0)) break;
-        if (pair > prev) pair = prev;
-        prev = pair;
-        tau += 2.0 * pair;
+  const double dn = (double)n;
+  for (int g = 0; g < P; ++g) {
+    // local chains of group g: [g·K, (g+1)·K) ∩ [off, off + B)
+    const int64_t lo = K ? std::max<int64_t>((int64_t)g * K, off) : 0, hi = K ? std::min<int64_t>((int64_t)(g + 1) * K, off + B) : B;
+    const double m = 2.0 * (double)std::max<int64_t>(hi - lo, 0);
+    for (int d = 0; d < D; ++d) {
+      const size_t o = (size_t)g * D + d;
+      if (m == 0) { if (rhat) rhat[o] = dm_nan(); if (ess) ess[o] = dm_nan(); continue; }
+      const double* a = &acc[o * (L + 3)];
+      const double mean_var = a[2] / m * dn / (dn - 1.0);                    // W: mean within-sequence variance (n − 1)
+      const double var_means = m > 1 ? (a[1] - a[0] * a[0] / m) / (m - 1.0) : 0.0;
+      const double var_plus = mean_var * (dn - 1.0) / dn + var_means;        // (n−1)/n·W + B/n
+      if (rhat) rhat[o] = std::sqrt(var_plus / mean_var);
+      if (ess) {
+        // Geyer's initial monotone sequence on ρ̂_t = 1 − (W − mean acov_t) / var⁺, pairs (ρ̂_2k + ρ̂_2k+1)
+        double tau = 0.0, prev = 1e300;
+        for (int t = 0; t + 1 <= L; t += 2) {
+          const double r0 = 1.0 - (mean_var - a[2 + t] / m) / var_plus, r1 = 1.0 - (mean_var - a[3 + t] / m) / var_plus;
+          double pair = r0 + r1;
+          if (!(pair > 0.0)) break;
+          if (pair > prev) pair = prev;
+          prev = pair;
+          tau += 2.0 * pair;
+        }
+        tau -= 1.0;
+        if (tau < 1.0 / std::log10(m * dn)) tau = 1.0 / std::log10(m * dn);   // cap of the super-efficient case (Stan: ESS ≤ S·log10 S)
+        ess[o] = m * dn / tau;
       }
-      tau -= 1.0;
-      if (tau < 1.0 / std::log10(m * dn)) tau = 1.0 / std::log10(m * dn);   // cap of the super-efficient case (Stan: ESS ≤ S·log10 S)
-      ess[d] = m * dn / tau;
     }
   }
   return DHMC_OK;
+}
+int dhmc_ess_rhat_dev(dhmc_handle* h, const double* draws_dev, int32_t N, int32_t max_lag, double* rhat, double* ess) {
+  if (!h || !draws_dev || N < 4 || (!rhat && !ess)) return DHMC_EARG;
+  return ess_rhat_groups(h, draws_dev, N, max_lag, 0, 1, rhat, ess);
+}
+int dhmc_ess_rhat_problems_dev(dhmc_handle* h, const double* draws_dev, int32_t N, int32_t max_lag, double* rhat, double* ess) {
+  if (!h || !draws_dev || N < 4 || (!rhat && !ess)) return DHMC_EARG;
+  if (!h->batch_k) { h->err = "dhmc_ess_rhat_problems_dev: the handle holds no problem batch (dhmc_set_problems)"; return DHMC_EARG; }
+  return ess_rhat_groups(h, draws_dev, N, max_lag, h->batch_k, (int)h->batch_p, rhat, ess);
 }
 int dhmc_acceptance_quantiles_dev(dhmc_handle* h, const dhmc_tree_stats* stats_dev, int32_t N, const double* probs,
                                   int32_t nprobs, double* out) {

@@ -64,6 +64,11 @@ struct KArgs {
   double* mean_out;             // pooled Symmetric stage: the window mean of every chain [B][D] (else null)
   int pooled;                   // the current dense metric is shared by every group of 8 chains (DHMC_METRIC_SYMMETRIC_POOLED)
   const double* minv_pad;       // tensor-core mat-vec: padded M⁻¹ [B][⌈D/32⌉·32][tma_xs(D)]
+  // problem batches (dhmc_set_problems): global chain g reads problem g / batch_k, whose blocks start at
+  // mparams, lX, lXt, ly, lXp + problem · (stride of that array); batch_k = 0: one problem for every chain.
+  // Global ids of a batch stay below 2^31 (host-checked), so the problem index is a 32-bit division.
+  int batch_k;
+  size_t s_mparams, s_lX, s_lXt, s_ly, s_lXp;    // doubles
 };
 
 // Register budget: minimum resident CTAs per SM the compiler must allow for.
@@ -134,8 +139,9 @@ __device__ __forceinline__ int next_chain_group(B& b, unsigned* counter, int beg
   if (b.lane == 0) c = begin + (int)atomicAdd(counter, 1u);
   return __shfl_sync(0xffffffffu, c, 0);
 }
-// pooled metric: the whole CTA (8 chains = one metric group) takes group g; warp w runs chain begin + 8·g + w.  All warps
-// arrive here together (they left the previous group through coop_finish), so a CTA barrier is safe.
+// pooled metric or problem batch: the whole CTA (8 chains = one metric group / 8 chains of one problem) takes group g; warp w
+// runs chain begin + 8·g + w.  All warps arrive here together (they left the previous group through coop_finish), so a CTA
+// barrier is safe.
 template <class B>
 __device__ __forceinline__ int next_pooled_group(B& b, unsigned* counter, int begin) {
   int* slot = reinterpret_cast<int*>(b.cb_shared + 96);
@@ -168,6 +174,15 @@ __device__ __forceinline__ void load_chain(DeviceBackend<EPL, FAM, W, DN, G, DP>
     b.rhoL[e] = 0.0;
   }
   b.lq = a.lq[c];
+  if (a.batch_k) {       // problem batch: the parameter block of this chain's problem (uniform over the chain's threads)
+    const size_t pr = (unsigned)(a.chain_offset + c) / (unsigned)a.batch_k;
+    b.mparams = a.mparams + pr * a.s_mparams;
+    b.lX = a.lX + pr * a.s_lX; b.lXt = a.lXt + pr * a.s_lXt; b.ly = a.ly + pr * a.s_ly;
+    // packed groups: the CTA's 8 chains are one problem (group fetch, host-checked 8-alignment), so every warp points the
+    // shared rounds at the same X.  No bulk copy outlives a round — coop_core_tma issues blocks 0, 1 and then b + 2 only
+    // while b + 2 < nblk, and waits on every one of them before its closing barrier — so X may change between groups.
+    if constexpr (G > 1) b.lXp = a.lXp + pr * a.s_lXp;
+  }
   const size_t dd = (size_t)a.D * a.D;
   if (a.covt) b.covt = a.covt + (size_t)c * dd;
   b.mean_out = a.mean_out ? a.mean_out + (size_t)c * a.D : nullptr;
@@ -224,7 +239,7 @@ __global__ void __launch_bounds__(32 * W * G, G > 1 ? 1 : min_ctas(W, EPL)) k_nu
   for (;;) {
     int c;
     if constexpr (G > 1) {
-      if (a.pooled) c = next_pooled_group(b, a.counter, a.chain_begin);    // the CTA takes a whole metric group
+      if (a.pooled || a.batch_k) c = next_pooled_group(b, a.counter, a.chain_begin);   // the CTA takes a whole metric group / 8 chains of one problem
       else c = next_chain_group(b, a.counter, a.chain_begin);
     } else {
       c = next_chain(a.counter, s_misc, a.chain_begin);
@@ -246,7 +261,7 @@ __global__ void __launch_bounds__(32 * W * G, G > 1 ? 1 : min_ctas(W, EPL)) k_nu
       if (m.status) atomicOr(a.status + c, m.status);
       atomicAdd(a.total_steps, (unsigned long long)m.steps_out);
     }
-    if constexpr (G > 1) { if (a.pooled) b.coop_finish(); }     // pooled metric: the group leaves together, then the CTA takes the next one
+    if constexpr (G > 1) { if (a.pooled || a.batch_k) b.coop_finish(); }     // group fetch: the group leaves together, then the CTA takes the next one
   }
   b.coop_finish();
 }
@@ -262,7 +277,7 @@ __global__ void __launch_bounds__(32 * W * G, G > 1 ? 1 : min_ctas(W, EPL)) k_se
   for (;;) {
     int c;
     if constexpr (G > 1) {
-      if (a.pooled) c = next_pooled_group(b, a.counter, a.chain_begin);
+      if (a.pooled || a.batch_k) c = next_pooled_group(b, a.counter, a.chain_begin);
       else c = next_chain_group(b, a.counter, a.chain_begin);
     } else {
       c = next_chain(a.counter, s_misc, a.chain_begin);
@@ -276,7 +291,7 @@ __global__ void __launch_bounds__(32 * W * G, G > 1 ? 1 : min_ctas(W, EPL)) k_se
       a.eps[c] = eps;
       if (m.status) atomicOr(a.status + c, m.status);
     }
-    if constexpr (G > 1) { if (a.pooled) b.coop_finish(); }
+    if constexpr (G > 1) { if (a.pooled || a.batch_k) b.coop_finish(); }
   }
   b.coop_finish();
 }

@@ -103,6 +103,17 @@ int dhmc_get_layout(dhmc_handle* h, int32_t* threads_per_chain, int32_t* elems_p
 /* params: DIAG_NORMAL [mu(D), prec(D)]; LOGISTIC [N, X row-major (N*D), y (N)]; STD_NORMAL / FUNNEL: n == 0;
  * USER: any block of doubles, handed to the user's formulas as `params`. */
 int dhmc_set_problem(dhmc_handle* h, const double* params, size_t n);
+/* Problem batch: n_problems posteriors of the handle's family and dimension, each with its own parameter block, on one
+ * handle.  Problem p's block is params + p*n_per_problem, in the format of dhmc_set_problem (LOGISTIC: every block has the
+ * same N).  Global chain g samples problem g / chains_per_problem, so chains [p*K, (p+1)*K) of a batch are bit-identical to
+ * a single-problem handle that holds problem p with chain_offset = p*K (K = chains_per_problem); every rank of a sharded
+ * run holds all blocks.  The handle's global chain ids must all be < n_problems * chains_per_problem.  Packed LOGISTIC
+ * handles (automatic layout, dim <= 256) run 8 chains of one problem per CTA: chains_per_problem, chain_offset and
+ * n_chains must be multiples of 8 (threads_per_chain = 32 lifts this).  STD_NORMAL and FUNNEL have no parameters and
+ * refuse a batch.  Everything is checked before anything is allocated; on any error the previous problem stays in
+ * effect.  dhmc_set_problem returns the handle to one problem. */
+int dhmc_set_problems(dhmc_handle* h, const double* params, size_t n_per_problem, int64_t n_problems,
+                      int64_t chains_per_problem);
 /* The user's own ℓ (LogDensityProblems.logdensity_and_gradient, call site hamiltonian.jl:204) as device code: a library
  * built from a model header (include/dhmc_models.h "the model header contract"; `make -C dynamichmc.jl_b200/csrc user
  * USER_HEADER=… USER_LIB=…`) carries family DHMC_FAMILY_USER (and only that family).  Copies the model's DHMC_USER_NAME
@@ -202,6 +213,11 @@ int dhmc_tree_summary_dev(dhmc_handle* h, const dhmc_tree_stats* stats_dev, int3
  * correctness tests compute with MCMCDiagnosticTools.ess_rhat (test/sample-correctness_utilities.jl:40-43).
  * rhat, ess: host [D], either may be NULL. */
 int dhmc_ess_rhat_dev(dhmc_handle* h, const double* draws_dev, int32_t N, int32_t max_lag, double* rhat, double* ess);
+/* The same per (problem, parameter) of a problem batch, over each problem's local chains (dhmc_ess_rhat_dev pools all
+ * chains, which mixes the problems).  rhat, ess: host [D, n_problems] column-major; a problem without a local chain
+ * gets NaN. */
+int dhmc_ess_rhat_problems_dev(dhmc_handle* h, const double* draws_dev, int32_t N, int32_t max_lag, double* rhat,
+                               double* ess);
 /* Quantiles of the acceptance rates (Diagnostics.summarize_tree_statistics: a_quantiles at 0.05 … 0.95,
  * diagnostics.jl:35,100-106) of a device statistics buffer [N, B], from a 4096-bin histogram (resolution 2.4e-4). */
 int dhmc_acceptance_quantiles_dev(dhmc_handle* h, const dhmc_tree_stats* stats_dev, int32_t N, const double* probs,

@@ -127,6 +127,27 @@ function bind_user_library(path::AbstractString; name = Symbol("B200HMC_", repla
         getfield(outer, :B200HMC)
     end
 end
+"""
+Many posteriors on one handle (dhmc_set_problems): `problems` share family and dimension and have parameter blocks of equal
+length (logistic regression: the same N); global chain g samples problem g ÷ K.  Built by
+`mcmc_with_warmup(seed, problems, N; chains_per_problem = K)`.
+"""
+struct ProblemBatch <: DeviceLogDensity
+    problems::Vector{DeviceLogDensity}; K::Int
+    function ProblemBatch(problems::AbstractVector, K::Integer)
+        isempty(problems) && throw(ArgumentError("a batch needs at least one problem"))
+        K ≥ 1 || throw(ArgumentError("chains_per_problem ≥ 1"))
+        f, D = family(first(problems)), LogDensityProblems.dimension(first(problems))
+        all(ℓ -> family(ℓ) == f && LogDensityProblems.dimension(ℓ) == D, problems) ||
+            throw(ArgumentError("every problem of a batch has the same family and dimension"))
+        all(ℓ -> length(params(ℓ)) == length(params(first(problems))), problems) ||
+            throw(ArgumentError("every problem of a batch has a parameter block of the same length (logistic: the same N)"))
+        new(collect(DeviceLogDensity, problems), Int(K))
+    end
+end
+family(b::ProblemBatch) = family(first(b.problems))
+params(b::ProblemBatch) = reduce(vcat, params.(b.problems))
+LogDensityProblems.dimension(b::ProblemBatch) = LogDensityProblems.dimension(first(b.problems))
 params(ℓ::DiagNormal) = vcat(ℓ.μ, 1 ./ ℓ.σ²)
 params(ℓ::LogisticRegression) = vcat(Float64(size(ℓ.X, 1)), vec(permutedims(ℓ.X)), ℓ.y)   # [N, X row-major, y]
 LogDensityProblems.capabilities(::Type{<:DeviceLogDensity}) = LogDensityProblems.LogDensityOrder{1}()
@@ -184,7 +205,12 @@ function _initialize(seed, ℓ::DeviceLogDensity, chains, initialization, algori
     h = Handle(Config(device, family(ℓ), D, chains, chain_offset, seed, algorithm.max_depth, 0,
                       algorithm.min_Δ, 0, 0))
     p = params(ℓ)
-    _ck(h, ccall((:dhmc_set_problem, LIB), Cint, (Ptr{Cvoid}, Ptr{Float64}, Csize_t), h.ptr, p, length(p)))
+    if ℓ isa ProblemBatch
+        _ck(h, ccall((:dhmc_set_problems, LIB), Cint, (Ptr{Cvoid}, Ptr{Float64}, Csize_t, Int64, Int64),
+                     h.ptr, p, length(p) ÷ length(ℓ.problems), length(ℓ.problems), ℓ.K))
+    else
+        _ck(h, ccall((:dhmc_set_problem, LIB), Cint, (Ptr{Cvoid}, Ptr{Float64}, Csize_t), h.ptr, p, length(p)))
+    end
     init = NamedTuple(initialization)
     if haskey(init, :κ)
         M⁻¹ = init.κ.M⁻¹
@@ -258,6 +284,22 @@ function mcmc_with_warmup(seed::Integer, ℓ::DeviceLogDensity, N::Integer; kwar
     r = mcmc_keep_warmup(seed, ℓ, N; kwargs...)
     (; κ, ϵ) = r.final_warmup_state
     [(; r.inference[k]..., κ = κ[k], ϵ = ϵ[k]) for k in eachindex(r.inference)]
+end
+
+# ---- problem batches: P posteriors, K chains each, one handle (dhmc_set_problems) ----------------------------
+"The results of P problems on one handle: element p is the vector of its K chains' NamedTuples (as `mcmc_with_warmup`)."
+function mcmc_with_warmup(seed::Integer, problems::AbstractVector{<:DeviceLogDensity}, N::Integer; chains_per_problem::Integer,
+                          kwargs...)
+    b = ProblemBatch(problems, chains_per_problem)
+    r = mcmc_with_warmup(seed, b, N; chains = length(problems) * b.K, kwargs...)
+    [r[(p - 1) * b.K + 1:p * b.K] for p in eachindex(problems)]
+end
+"split-R̂ and ESS per (parameter, problem) of a batch handle's DEVICE draws [D, N, chains] (dhmc_ess_rhat_problems_dev): [D, P]."
+function ess_rhat_problems(h::Handle, draws_dev::Ptr{Float64}, N::Integer, P::Integer; max_lag::Integer = 0)
+    rhat, ess = Matrix{Float64}(undef, h.D, P), Matrix{Float64}(undef, h.D, P)
+    _ck(h, ccall((:dhmc_ess_rhat_problems_dev, LIB), Cint, (Ptr{Cvoid}, Ptr{Float64}, Int32, Int32, Ptr{Float64}, Ptr{Float64}),
+                 h.ptr, draws_dev, N, max_lag, rhat, ess))
+    (; rhat, ess)
 end
 
 # ---- mcmc_steps / mcmc_next_step — src/mcmc.jl:335-351: stepwise sampling at the adapted (κ, ϵ) -----
