@@ -18,7 +18,8 @@ tree_stats_dtype = np.dtype(
      ("acceptance_rate", "<f8"), ("steps", "<i8"), ("directions", "<u4"), ("pad", "<u4")])
 
 EXPORTS = [
-    "dhmc_create", "dhmc_destroy", "dhmc_last_error", "dhmc_get_layout", "dhmc_set_problem", "dhmc_set_problems", "dhmc_user_family_name",
+    "dhmc_create", "dhmc_destroy", "dhmc_last_error", "dhmc_get_layout", "dhmc_set_problem", "dhmc_set_problems", "dhmc_set_problems_ragged",
+    "dhmc_user_family_name",
     "dhmc_family_available",
     "dhmc_set_position", "dhmc_random_position", "dhmc_set_metric", "dhmc_set_metric_dense",
     "dhmc_get_metric_dense", "dhmc_metric_is_dense", "dhmc_set_stepsize",

@@ -244,6 +244,16 @@ class ProblemBatch:
     the host; hand it to Engine / mcmc_with_warmup in place of ℓ."""
 
     def __init__(self, problems, chains_per_problem):
+        blocks = self._check_problems(problems, chains_per_problem)
+        if self.family == L.FAMILY_LOGISTIC:
+            _argcheck(all(b[0] == blocks[0][0] for b in blocks), "every logistic problem of a batch has the same N")
+        _argcheck(all(b.size == blocks[0].size for b in blocks), "every problem of a batch has a parameter block of the same length")
+        _argcheck(blocks[0].size >= 1, "the problems have empty parameter blocks")
+        self.block_size = blocks[0].size
+        self._params = np.concatenate(blocks)
+
+    def _check_problems(self, problems, chains_per_problem):
+        """the checks every batch shares (family, dimension, library, chain count); returns the parameter blocks"""
         problems = list(problems)
         _argcheck(len(problems) >= 1, "a batch needs at least one problem")
         _argcheck(all(isinstance(x, DeviceLogDensity) for x in problems), "problems: DeviceLogDensity objects")
@@ -258,14 +268,8 @@ class ProblemBatch:
         self.library_path = getattr(first, "library_path", None)
         _argcheck(all(getattr(x, "library_path", None) == self.library_path for x in problems),
                   "every problem of a batch lives in the same user-model library")
-        blocks = [np.ascontiguousarray(x.params(), float).ravel() for x in problems]
-        if self.family == L.FAMILY_LOGISTIC:
-            _argcheck(all(b[0] == blocks[0][0] for b in blocks), "every logistic problem of a batch has the same N")
-        _argcheck(all(b.size == blocks[0].size for b in blocks), "every problem of a batch has a parameter block of the same length")
-        _argcheck(blocks[0].size >= 1, "the problems have empty parameter blocks")
         self.problems = problems
-        self.block_size = blocks[0].size
-        self._params = np.concatenate(blocks)
+        return [np.ascontiguousarray(x.params(), float).ravel() for x in problems]
 
     @property
     def n_problems(self):
@@ -292,6 +296,24 @@ class ProblemBatch:
         K = self.chains_per_problem
         lo, hi = max(p * K - chain_offset, 0), min((p + 1) * K - chain_offset, chains)
         return lo, max(lo, hi)
+
+
+class RaggedProblemBatch(ProblemBatch):
+    """A ProblemBatch whose parameter blocks may differ in length (dhmc_set_problems_ragged): logistic regressions with
+    their own number of observations each — one fit per hospital, school or customer, or the folds of a k-fold split.
+    Each problem's data take device memory of their own size, and a packed CTA streams only its problem's rows, where
+    padding every problem to the largest N would cost max N / mean N of the useful work.  A user model's formulas do not
+    receive the length of their block: a model that needs it stores it in the block.  Problems of equal length are
+    accepted too and sample exactly as the ProblemBatch of the same problems.  Problem p's block is
+    params()[block_offsets[p]:block_offsets[p + 1]] (block_offsets: [P + 1], size_t)."""
+
+    def __init__(self, problems, chains_per_problem):
+        blocks = self._check_problems(problems, chains_per_problem)
+        _argcheck(all(b.size >= 1 for b in blocks), "every problem of a batch needs a non-empty parameter block")
+        self.block_size = None
+        self.block_offsets = np.zeros(len(blocks) + 1, dtype=np.dtype(C.c_size_t))
+        np.cumsum([b.size for b in blocks], out=self.block_offsets[1:])
+        self._params = np.concatenate(blocks)
 
 
 # ------------------------------------------------------------------ algorithm structs
@@ -415,13 +437,16 @@ class Engine:
         self._set_problem(ℓ)
 
     def _set_problem(self, ℓ):
-        """dhmc_set_problem, or dhmc_set_problems for a ProblemBatch.  On an error the handle keeps its previous problem."""
+        """dhmc_set_problem, or dhmc_set_problems(_ragged) for a (Ragged)ProblemBatch.  On an error the handle keeps its previous problem."""
         if self.ℓ is not ℓ:                              # replacing the problem of an existing handle
             _argcheck(ℓ.family == self.ℓ.family and int(ℓ.dimension()) == self.D, "same family and dimension as the handle")
             _argcheck(getattr(ℓ, "library_path", None) == getattr(self.ℓ, "library_path", None),
                       "a user model of the handle's own library")
         pr = np.ascontiguousarray(ℓ.params(), float)
-        if isinstance(ℓ, ProblemBatch):
+        if isinstance(ℓ, RaggedProblemBatch):
+            self._ck(self._lib.dhmc_set_problems_ragged(self._h, L.ptr(pr), L.ptr(ℓ.block_offsets), C.c_int64(ℓ.n_problems),
+                                                        C.c_int64(ℓ.chains_per_problem)))
+        elif isinstance(ℓ, ProblemBatch):
             self._ck(self._lib.dhmc_set_problems(self._h, L.ptr(pr), C.c_size_t(ℓ.block_size), C.c_int64(ℓ.n_problems),
                                                  C.c_int64(ℓ.chains_per_problem)))
         else:

@@ -353,11 +353,11 @@ struct dhmc_handle {
   double* minv_pad = nullptr;       // packed groups on the tensor cores: zero-padded row blocks of every chain's M⁻¹
   double *lX = nullptr, *lXt = nullptr, *ly = nullptr, *lr = nullptr;   // logistic regression
   double* lXp = nullptr;            // … zero-padded row blocks of X for the tensor-core likelihood
-  int lN = 0, lLd = 0;
-  // problem batch (dhmc_set_problems): chains per problem (0 = one problem), problems, per-problem strides of the parameter
-  // arrays in doubles (mparams, lX, lXt, ly, lXp)
+  int lN = 0, lLd = 0;              // (a batch: lN is the largest N, the row length of the residual scratch lr)
+  // problem batch (dhmc_set_problems / _ragged): chains per problem (0 = one problem), problems, and the device table of
+  // per-problem descriptors (where each problem's blocks start in mparams, lX, lXt, ly, lXp; its N and leading dimension)
   int64_t batch_k = 0, batch_p = 0;
-  size_t s_mparams = 0, s_lX = 0, s_lXt = 0, s_ly = 0, s_lXp = 0;
+  ProblemDesc* problems = nullptr;
   int reg_ctas[2] = {0, 0};         // occupancy of k_nuts (diag, dense)
   size_t smem_sm = 0, smem_cta_max = 0;
   ncclComm_t comm = nullptr;        // multi-GPU: one communicator per handle (dhmc_comm_init)
@@ -468,8 +468,7 @@ static KArgs base_args(dhmc_handle* h) {
   a.minv_dense = h->minv_dense; a.wt = h->wt; a.covt = nullptr; a.minv_pad = h->minv_pad; a.mean_out = nullptr; a.pooled = h->pooled ? 1 : 0;
   a.xs_doubles = needs_staging(h) ? (int)((size_t)h->T * h->EPL) : 0;
   a.lX = h->lX; a.lXt = h->lXt; a.ly = h->ly; a.lr = h->lr; a.lN = h->lN; a.lLd = h->lLd; a.lXp = h->lXp;
-  a.batch_k = (int)h->batch_k;
-  a.s_mparams = h->s_mparams; a.s_lX = h->s_lX; a.s_lXt = h->s_lXt; a.s_ly = h->s_ly; a.s_lXp = h->s_lXp;
+  a.batch_k = (int)h->batch_k; a.problems = h->problems;
   return a;
 }
 
@@ -563,7 +562,7 @@ int dhmc_destroy(dhmc_handle* h) {
   cudaFree(h->mparams); cudaFree(h->status); cudaFree(h->scratch); cudaFree(h->counter);
   cudaFree(h->total_steps);
   cudaFree(h->minv_dense); cudaFree(h->wt); cudaFree(h->covt); cudaFree(h->dense_tmp); cudaFree(h->minv_pad); cudaFree(h->mean_pool);
-  cudaFree(h->lX); cudaFree(h->lXt); cudaFree(h->ly); cudaFree(h->lr); cudaFree(h->lXp);
+  cudaFree(h->lX); cudaFree(h->lXt); cudaFree(h->ly); cudaFree(h->lr); cudaFree(h->lXp); cudaFree(h->problems);
   cudaFree(h->tmp_b); cudaFree(h->tmp_bd); cudaFree(h->tmp_dir);
   for (void* r : h->registered) cudaHostUnregister(r);
   if (h->comm) dhmc_comm_destroy(h);
@@ -696,7 +695,7 @@ int dhmc_user_family_name(char* name, size_t cap) {
 
 static void clear_batch(dhmc_handle* h) {
   h->batch_k = h->batch_p = 0;
-  h->s_mparams = h->s_lX = h->s_lXt = h->s_ly = h->s_lXp = 0;
+  cudaFree(h->problems); h->problems = nullptr;
 }
 
 int dhmc_set_problem(dhmc_handle* h, const double* params, size_t n) {
@@ -752,29 +751,103 @@ int dhmc_set_problem(dhmc_handle* h, const double* params, size_t n) {
   return DHMC_OK;
 }
 
-// P problems of the handle's family and dimension, each with its own parameter block; global chain g samples problem
-// g / chains_per_problem.  Everything is validated before anything is allocated, and the new arrays are complete before
-// they replace the current ones: on any error the previous problem (batch or not) stays in effect.
+// The checks every problem batch shares (dhmc_set_problems, dhmc_set_problems_ragged); `who` names the entry point in the
+// messages.
+static int check_batch(dhmc_handle* h, const char* who, bool have_blocks, int64_t P, int64_t K) {
+  const int fam = h->cfg.family;
+  const int64_t off = h->cfg.chain_offset, B = h->cfg.n_chains;
+  auto fail = [&](const char* m) { h->err = std::string(who) + ": " + m; return DHMC_EARG; };
+  if (fam != DHMC_FAMILY_DIAG_NORMAL && fam != DHMC_FAMILY_LOGISTIC && fam != DHMC_FAMILY_USER)
+    return fail("this family has no parameters (a batch of it would be one problem)");
+  if (P < 1 || K < 1 || !have_blocks) return fail("n_problems >= 1, chains_per_problem >= 1 and a parameter block per problem");
+  if (P > INT32_MAX / K) return fail("n_problems * chains_per_problem < 2^31");
+  if (off < 0 || off + B > P * K)
+    return fail("the handle's chains [chain_offset, chain_offset + n_chains) lie beyond n_problems * chains_per_problem");
+  if (h->G > 1 && (K % 8 != 0 || off % 8 != 0 || B % 8 != 0))
+    return fail("packed chain groups (logistic, automatic layout, dim <= 256) run 8 chains of one problem per CTA: "
+                "chains_per_problem, chain_offset and n_chains must be multiples of 8 (threads_per_chain=32 runs one chain per CTA without this condition)");
+  return DHMC_OK;
+}
+
+// Installs P validated blocks (problem p: params[offs[p] .. offs[p+1])), each sampled by K chains.  Every problem gets arrays of
+// its own size, back to back, and a descriptor that says where they start.  The new arrays are complete before they replace
+// the current ones: on any error the previous problem (batch or not) stays in effect.
+static int install_batch(dhmc_handle* h, const double* params, const std::vector<size_t>& offs, int64_t P, int64_t K) {
+  const int fam = h->cfg.family;
+  const size_t D = (size_t)h->cfg.dim, Pz = (size_t)P;
+  const size_t xs = fam == DHMC_FAMILY_LOGISTIC ? (size_t)tma_xs((int)D) : 0;
+  std::vector<ProblemDesc> desc(Pz);
+  size_t tX = 0, tXt = 0, ty = 0, tXp = 0, maxN = 0;
+  for (size_t p = 0; p < Pz; ++p) {
+    ProblemDesc& d = desc[p];
+    d = ProblemDesc{};
+    if (fam != DHMC_FAMILY_LOGISTIC) { d.mparams = offs[p]; continue; }
+    const size_t N = (size_t)params[offs[p]];
+    const size_t ld = (N + 1) & ~(size_t)1;                     // even leading dimension: 16-byte aligned row segments
+    const size_t rows = (N + kTmaRows - 1) / kTmaRows * kTmaRows; // whole row blocks of [32][xs] for the bulk copies
+    d.X = tX; d.Xt = tXt; d.y = ty; d.Xp = h->G > 1 ? tXp : 0; d.N = (int)N; d.ld = (int)ld;
+    tX += N * D; tXt += ld * D; ty += N; tXp += rows * xs;
+    maxN = std::max(maxN, N);
+    if (d.Xt % 2 != 0 || (h->G > 1 && d.Xp % (kTmaRows * xs) != 0)) {
+      h->err = "problem batch: misaligned problem base in X^T or padded X (internal error)"; return DHMC_ECUDA;
+    }
+  }
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->stream));
+  double *mp = nullptr, *X = nullptr, *Xt = nullptr, *y = nullptr, *Xp = nullptr, *lr = nullptr;
+  ProblemDesc* dd = nullptr;
+  auto drop = [&] { cudaFree(mp); cudaFree(X); cudaFree(Xt); cudaFree(y); cudaFree(Xp); cudaFree(lr); cudaFree(dd); };
+#define CKB(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { h->err = std::string(#call) + ": " + cudaGetErrorString(e_); \
+    cudaStreamSynchronize(h->stream); drop(); return e_ == cudaErrorMemoryAllocation ? DHMC_ENOMEM : DHMC_ECUDA; } } while (0)
+  CKB(cudaMalloc(&dd, sizeof(ProblemDesc) * Pz));
+  CKB(cudaMemcpyAsync(dd, desc.data(), sizeof(ProblemDesc) * Pz, cudaMemcpyHostToDevice, h->stream));
+  if (fam == DHMC_FAMILY_LOGISTIC) {
+    // per problem: X [N][D], Xᵀ [D][ld], y [N] and, for packed groups, the zero-padded row blocks [rows][xs]; one residual
+    // scratch of rows of the largest N
+    CKB(cudaMalloc(&X, sizeof(double) * tX));
+    CKB(cudaMalloc(&Xt, sizeof(double) * tXt));
+    CKB(cudaMalloc(&y, sizeof(double) * ty));
+    CKB(cudaMalloc(&lr, sizeof(double) * maxN * lr_rows(h)));
+    if (h->G > 1) CKB(cudaMalloc(&Xp, sizeof(double) * tXp));
+    for (size_t p = 0; p < Pz; ++p) {
+      const double* blk = params + offs[p];
+      const ProblemDesc& d = desc[p];
+      const size_t N = (size_t)d.N;
+      CKB(cudaMemcpyAsync(X + d.X, blk + 1, sizeof(double) * N * D, cudaMemcpyHostToDevice, h->stream));
+      CKB(cudaMemcpyAsync(y + d.y, blk + 1 + N * D, sizeof(double) * N, cudaMemcpyHostToDevice, h->stream));
+      k_transpose<<<1024, 256, 0, h->stream>>>(X + d.X, Xt + d.Xt, N, D, (size_t)d.ld);
+      if (Xp) k_pad_rows<<<1024, 256, 0, h->stream>>>(X + d.X, Xp + d.Xp, N, D, (N + kTmaRows - 1) / kTmaRows * kTmaRows, xs);
+      h->launches += Xp ? 2 : 1;
+    }
+  } else {
+    CKB(cudaMalloc(&mp, sizeof(double) * offs[Pz]));
+    CKB(cudaMemcpyAsync(mp, params, sizeof(double) * offs[Pz], cudaMemcpyHostToDevice, h->stream));
+  }
+  CKB(cudaGetLastError());
+  CKB(cudaStreamSynchronize(h->stream));
+#undef CKB
+  if (fam == DHMC_FAMILY_LOGISTIC) {
+    cudaFree(h->lX); cudaFree(h->lXt); cudaFree(h->ly); cudaFree(h->lr); cudaFree(h->lXp);
+    h->lX = X; h->lXt = Xt; h->ly = y; h->lr = lr; h->lXp = Xp;
+    h->lN = (int)maxN; h->lLd = desc[0].ld;    // a chain's own N and ld come from its descriptor
+  } else {
+    cudaFree(h->mparams);
+    h->mparams = mp;
+  }
+  cudaFree(h->problems);
+  h->problems = dd;
+  h->batch_k = K; h->batch_p = P;
+  return DHMC_OK;
+}
+
+// P problems of the handle's family and dimension, each with its own parameter block of n doubles; global chain g samples
+// problem g / chains_per_problem.  Everything is validated before anything is allocated.
 int dhmc_set_problems(dhmc_handle* h, const double* params, size_t n, int64_t P, int64_t K) {
   if (!h) return DHMC_EARG;
   const int fam = h->cfg.family;
   const size_t D = (size_t)h->cfg.dim;
-  const int64_t off = h->cfg.chain_offset, B = h->cfg.n_chains;
-  if (fam != DHMC_FAMILY_DIAG_NORMAL && fam != DHMC_FAMILY_LOGISTIC && fam != DHMC_FAMILY_USER) {
-    h->err = "dhmc_set_problems: this family has no parameters (a batch of it would be one problem)"; return DHMC_EARG;
-  }
-  if (P < 1 || K < 1 || !params || n < 1) { h->err = "dhmc_set_problems: n_problems >= 1, chains_per_problem >= 1 and a parameter block per problem"; return DHMC_EARG; }
-  if (P * K > INT32_MAX) { h->err = "dhmc_set_problems: n_problems * chains_per_problem < 2^31"; return DHMC_EARG; }
-  if (off < 0 || off + B > P * K) {
-    h->err = "dhmc_set_problems: the handle's chains [chain_offset, chain_offset + n_chains) lie beyond n_problems * chains_per_problem";
-    return DHMC_EARG;
-  }
-  if (h->G > 1 && (K % 8 != 0 || off % 8 != 0 || B % 8 != 0)) {
-    h->err = "dhmc_set_problems: packed chain groups (logistic, automatic layout, dim <= 256) run 8 chains of one problem per CTA: "
-             "chains_per_problem, chain_offset and n_chains must be multiples of 8 (threads_per_chain=32 runs one chain per CTA without this condition)";
-    return DHMC_EARG;
-  }
-  size_t N = 0, ld = 0, rows = 0, xs = 0;
+  if (int rc = check_batch(h, "dhmc_set_problems", params && n >= 1, P, K)) return rc;
+  size_t N = 0;
   if (fam == DHMC_FAMILY_DIAG_NORMAL && n != 2 * D) { h->err = "dhmc_set_problems: DIAG_NORMAL blocks are [mu(D), prec(D)]"; return DHMC_EARG; }
   if (fam == DHMC_FAMILY_LOGISTIC) {
     N = params[0] >= 1 ? (size_t)params[0] : 0;
@@ -787,51 +860,37 @@ int dhmc_set_problems(dhmc_handle* h, const double* params, size_t n, int64_t P,
         if (!(yv >= 0.0 && yv <= 1.0)) { h->err = "dhmc_set_problems: logistic regression needs 0 <= y <= 1"; return DHMC_EARG; }
       }
     }
-    ld = (N + 1) & ~(size_t)1;
-    rows = (N + kTmaRows - 1) / kTmaRows * kTmaRows;
-    xs = (size_t)tma_xs((int)D);
   }
-  CK(cudaSetDevice(h->cfg.device));
-  CK(cudaStreamSynchronize(h->stream));
-  double *mp = nullptr, *X = nullptr, *Xt = nullptr, *y = nullptr, *Xp = nullptr, *lr = nullptr;
-  auto drop = [&] { cudaFree(mp); cudaFree(X); cudaFree(Xt); cudaFree(y); cudaFree(Xp); cudaFree(lr); };
-#define CKB(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { h->err = std::string(#call) + ": " + cudaGetErrorString(e_); \
-    cudaStreamSynchronize(h->stream); drop(); return e_ == cudaErrorMemoryAllocation ? DHMC_ENOMEM : DHMC_ECUDA; } } while (0)
-  const size_t Pz = (size_t)P;
-  if (fam == DHMC_FAMILY_LOGISTIC) {
-    // per problem: X [N][D], Xᵀ [D][ld], y [N] and, for packed groups, the zero-padded row blocks [rows][xs]
-    CKB(cudaMalloc(&X, sizeof(double) * Pz * N * D));
-    CKB(cudaMalloc(&Xt, sizeof(double) * Pz * ld * D));
-    CKB(cudaMalloc(&y, sizeof(double) * Pz * N));
-    CKB(cudaMalloc(&lr, sizeof(double) * N * lr_rows(h)));
-    if (h->G > 1) CKB(cudaMalloc(&Xp, sizeof(double) * Pz * rows * xs));
-    for (size_t p = 0; p < Pz; ++p) {
-      const double* blk = params + p * n;
-      CKB(cudaMemcpyAsync(X + p * N * D, blk + 1, sizeof(double) * N * D, cudaMemcpyHostToDevice, h->stream));
-      CKB(cudaMemcpyAsync(y + p * N, blk + 1 + N * D, sizeof(double) * N, cudaMemcpyHostToDevice, h->stream));
-      k_transpose<<<1024, 256, 0, h->stream>>>(X + p * N * D, Xt + p * ld * D, N, D, ld);
-      if (Xp) k_pad_rows<<<1024, 256, 0, h->stream>>>(X + p * N * D, Xp + p * rows * xs, N, D, rows, xs);
-      h->launches += Xp ? 2 : 1;
+  std::vector<size_t> offs((size_t)P + 1);
+  for (size_t p = 0; p <= (size_t)P; ++p) offs[p] = p * n;
+  return install_batch(h, params, offs, P, K);
+}
+
+// The same with blocks of different lengths: problem p's block is params[block_offsets[p] .. block_offsets[p+1]).
+int dhmc_set_problems_ragged(dhmc_handle* h, const double* params, const size_t* offs, int64_t P, int64_t K) {
+  if (!h) return DHMC_EARG;
+  const int fam = h->cfg.family;
+  const size_t D = (size_t)h->cfg.dim;
+  if (int rc = check_batch(h, "dhmc_set_problems_ragged", params && offs, P, K)) return rc;
+  auto fail = [&](const char* m) { h->err = std::string("dhmc_set_problems_ragged: ") + m; return DHMC_EARG; };
+  if (offs[0] != 0) return fail("block_offsets[0] must be 0");
+  for (int64_t p = 0; p < P; ++p)
+    if (offs[p + 1] <= offs[p]) return fail("block_offsets must strictly increase (every block holds at least one value)");
+  for (int64_t p = 0; p < P; ++p) {
+    const double* blk = params + offs[p];
+    const size_t len = offs[p + 1] - offs[p];
+    if (fam == DHMC_FAMILY_DIAG_NORMAL && len != 2 * D) return fail("DIAG_NORMAL blocks are [mu(D), prec(D)]");
+    if (fam != DHMC_FAMILY_LOGISTIC) continue;
+    const double v = blk[0];
+    if (!(v >= 1.0 && v < 2147483648.0 && v == std::floor(v))) return fail("a logistic block starts with its N, an integer with 1 <= N < 2^31");
+    const size_t N = (size_t)v;
+    if (len != 1 + N * D + N) return fail("logistic blocks are [N, X (N*D), y (N)]: a block's length disagrees with its N");
+    for (size_t i = 0; i < N; ++i) {
+      const double yv = blk[1 + N * D + i];
+      if (!(yv >= 0.0 && yv <= 1.0)) return fail("logistic regression needs 0 <= y <= 1");
     }
-  } else {
-    CKB(cudaMalloc(&mp, sizeof(double) * Pz * n));
-    CKB(cudaMemcpyAsync(mp, params, sizeof(double) * Pz * n, cudaMemcpyHostToDevice, h->stream));
   }
-  CKB(cudaGetLastError());
-  CKB(cudaStreamSynchronize(h->stream));
-#undef CKB
-  if (fam == DHMC_FAMILY_LOGISTIC) {
-    cudaFree(h->lX); cudaFree(h->lXt); cudaFree(h->ly); cudaFree(h->lr); cudaFree(h->lXp);
-    h->lX = X; h->lXt = Xt; h->ly = y; h->lr = lr; h->lXp = Xp;
-    h->lN = (int)N; h->lLd = (int)ld;
-    h->s_mparams = 0; h->s_lX = N * D; h->s_lXt = ld * D; h->s_ly = N; h->s_lXp = Xp ? rows * xs : 0;
-  } else {
-    cudaFree(h->mparams);
-    h->mparams = mp;
-    h->s_mparams = n; h->s_lX = h->s_lXt = h->s_ly = h->s_lXp = 0;
-  }
-  h->batch_k = K; h->batch_p = P;
-  return DHMC_OK;
+  return install_batch(h, params, std::vector<size_t>(offs, offs + P + 1), P, K);
 }
 
 static int eval_position(dhmc_handle* h, bool randomize) {

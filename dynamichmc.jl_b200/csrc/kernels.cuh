@@ -22,6 +22,15 @@
 namespace dhmc {
 
 // ------------------------------------------------------------------ kernel args
+// One problem of a batch: where its blocks start in the handle's arrays (doubles) and, for logistic regression, its
+// observations and the leading dimension of its Xᵀ.  Problems lie back to back, each with arrays of its own size; the
+// host keeps every Xᵀ base even and every padded-X base a multiple of 32·tma_xs(D) doubles (16-byte row segments, whole
+// row blocks for the bulk copies).
+struct ProblemDesc {
+  size_t mparams, X, Xt, y, Xp;
+  int N, ld;
+};
+
 struct KArgs {
   int D, B, T, W;
   unsigned long long seed;
@@ -56,7 +65,7 @@ struct KArgs {
   int xs_doubles;               // shared-memory staging vector (0 unless the dense arrays exist)
   const double *lX, *lXt, *ly;  // logistic regression data
   double* lr;                   // logistic scratch of one chain per CTA: [grid][lN] residuals (packed groups need none)
-  int lN, lLd;                  // observations, leading dimension of Xᵀ (even)
+  int lN, lLd;                  // observations (a batch: the largest N, the scratch row length), leading dimension of Xᵀ (even)
   const double* lXp;            // tensor-core likelihood: zero-padded row blocks of X
   int levels, ntab;             // deep kernels (max_depth > 12) only: stack entries per warp (max_depth + 1), slot-table entries;
                                 // all other kernels use the compile-time kStdLevels / kStdTab so that the offsets fold into immediates
@@ -64,11 +73,11 @@ struct KArgs {
   double* mean_out;             // pooled Symmetric stage: the window mean of every chain [B][D] (else null)
   int pooled;                   // the current dense metric is shared by every group of 8 chains (DHMC_METRIC_SYMMETRIC_POOLED)
   const double* minv_pad;       // tensor-core mat-vec: padded M⁻¹ [B][⌈D/32⌉·32][tma_xs(D)]
-  // problem batches (dhmc_set_problems): global chain g reads problem g / batch_k, whose blocks start at
-  // mparams, lX, lXt, ly, lXp + problem · (stride of that array); batch_k = 0: one problem for every chain.
-  // Global ids of a batch stay below 2^31 (host-checked), so the problem index is a 32-bit division.
+  // problem batches (dhmc_set_problems / _ragged): global chain g reads problem g / batch_k, described by problems[g / batch_k];
+  // batch_k = 0: one problem for every chain (problems is null).  Global ids of a batch stay below 2^31 (host-checked), so
+  // the problem index is a 32-bit division.
   int batch_k;
-  size_t s_mparams, s_lX, s_lXt, s_ly, s_lXp;    // doubles
+  const ProblemDesc* problems;
 };
 
 // Register budget: minimum resident CTAs per SM the compiler must allow for.
@@ -174,14 +183,16 @@ __device__ __forceinline__ void load_chain(DeviceBackend<EPL, FAM, W, DN, G, DP>
     b.rhoL[e] = 0.0;
   }
   b.lq = a.lq[c];
-  if (a.batch_k) {       // problem batch: the parameter block of this chain's problem (uniform over the chain's threads)
-    const size_t pr = (unsigned)(a.chain_offset + c) / (unsigned)a.batch_k;
-    b.mparams = a.mparams + pr * a.s_mparams;
-    b.lX = a.lX + pr * a.s_lX; b.lXt = a.lXt + pr * a.s_lXt; b.ly = a.ly + pr * a.s_ly;
+  if (a.batch_k) {       // problem batch: the blocks of this chain's problem (uniform over the chain's threads)
+    const ProblemDesc& pd = a.problems[(unsigned)(a.chain_offset + c) / (unsigned)a.batch_k];
+    b.mparams = a.mparams + pd.mparams;
+    b.lX = a.lX + pd.X; b.lXt = a.lXt + pd.Xt; b.ly = a.ly + pd.y;
+    b.lN = pd.N; b.lLd = pd.ld;       // (the per-CTA residual scratch keeps its stride: a.lN, the batch's largest N)
     // packed groups: the CTA's 8 chains are one problem (group fetch, host-checked 8-alignment), so every warp points the
-    // shared rounds at the same X.  No bulk copy outlives a round — coop_core_tma issues blocks 0, 1 and then b + 2 only
-    // while b + 2 < nblk, and waits on every one of them before its closing barrier — so X may change between groups.
-    if constexpr (G > 1) b.lXp = a.lXp + pr * a.s_lXp;
+    // shared rounds at the same X and derives the same block count from the same N.  No bulk copy outlives a round —
+    // coop_core_tma issues blocks 0, 1 and then b + 2 only while b + 2 < nblk, and waits on every one of them before its
+    // closing barrier — so X and N may change between groups.
+    if constexpr (G > 1) b.lXp = a.lXp + pd.Xp;
   }
   const size_t dd = (size_t)a.D * a.D;
   if (a.covt) b.covt = a.covt + (size_t)c * dd;

@@ -114,6 +114,16 @@ int dhmc_set_problem(dhmc_handle* h, const double* params, size_t n);
  * effect.  dhmc_set_problem returns the handle to one problem. */
 int dhmc_set_problems(dhmc_handle* h, const double* params, size_t n_per_problem, int64_t n_problems,
                       int64_t chains_per_problem);
+/* Ragged problem batch: the same with blocks of different lengths — problem p's block is
+ * params[block_offsets[p] .. block_offsets[p+1]), block_offsets[0] == 0 and the offsets strictly increase.  LOGISTIC:
+ * every block is [N_p, X_p (N_p*D), y_p (N_p)] with its own integer 1 <= N_p < 2^31 that matches the block's length
+ * (per-unit regressions with any number of rows each).  Each problem's data take space of their own size (sum of N_p,
+ * not n_problems * max N_p), and a packed CTA streams only its problem's row blocks.  USER: blocks of any positive
+ * length (the formulas do not receive the length: a model that needs it stores it in its block).  DIAG_NORMAL: every
+ * block is 2*D long.  Every other rule, including the bit-identity to single-problem handles, is that of
+ * dhmc_set_problems. */
+int dhmc_set_problems_ragged(dhmc_handle* h, const double* params, const size_t* block_offsets, int64_t n_problems,
+                             int64_t chains_per_problem);
 /* The user's own ℓ (LogDensityProblems.logdensity_and_gradient, call site hamiltonian.jl:204) as device code: a library
  * built from a model header (include/dhmc_models.h "the model header contract"; `make -C dynamichmc.jl_b200/csrc user
  * USER_HEADER=… USER_LIB=…`) carries family DHMC_FAMILY_USER (and only that family).  Copies the model's DHMC_USER_NAME

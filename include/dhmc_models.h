@@ -115,7 +115,10 @@ DHMC_HD double dhmc_logit_grad(double xtr, double beta) { return xtr - beta; }
  *   DHMC_HD double dhmc_user_logdensity(int D, const double* q, const double* S, const double* params);
  *   DHMC_HD double dhmc_user_grad(int i, int D, const double* q, const double* S, const double* params);
  *
- * `params` is the block of doubles handed to dhmc_set_problem (any length).  The sums are taken in the canonical
+ * `params` is the block of doubles handed to dhmc_set_problem (any length) — in a problem batch, the chain's own
+ * problem's block.  The formulas never receive the block's length: a model whose blocks differ in length from problem to
+ * problem (dhmc_set_problems_ragged: e.g. a different number of observations per unit) stores the length, or whatever
+ * it needs to find its data, in the block itself.  The sums are taken in the canonical
  * order (DESIGN.md §3); transcendental functions should come from dhmc_math.h (dm_exp, dm_log, dm_log1p, …) if the
  * device results are to equal the oracle's bit for bit — libm / libdevice calls work, but differ in the last ulp.
  * -Inf / non-finite values are handled by the sampler exactly as for the shipped families (hamiltonian.jl:202-217). */

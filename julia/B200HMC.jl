@@ -145,9 +145,29 @@ struct ProblemBatch <: DeviceLogDensity
         new(collect(DeviceLogDensity, problems), Int(K))
     end
 end
-family(b::ProblemBatch) = family(first(b.problems))
-params(b::ProblemBatch) = reduce(vcat, params.(b.problems))
-LogDensityProblems.dimension(b::ProblemBatch) = LogDensityProblems.dimension(first(b.problems))
+"""
+A problem batch whose parameter blocks may differ in length (dhmc_set_problems_ragged): logistic regressions with their own
+number of observations each.  Each problem's data take device memory of their own size.  `mcmc_with_warmup(seed, problems, N;
+chains_per_problem = K)` builds one when the blocks differ in length.
+"""
+struct RaggedProblemBatch <: DeviceLogDensity
+    problems::Vector{DeviceLogDensity}; K::Int
+    function RaggedProblemBatch(problems::AbstractVector, K::Integer)
+        isempty(problems) && throw(ArgumentError("a batch needs at least one problem"))
+        K ≥ 1 || throw(ArgumentError("chains_per_problem ≥ 1"))
+        f, D = family(first(problems)), LogDensityProblems.dimension(first(problems))
+        all(ℓ -> family(ℓ) == f && LogDensityProblems.dimension(ℓ) == D, problems) ||
+            throw(ArgumentError("every problem of a batch has the same family and dimension"))
+        all(ℓ -> !isempty(params(ℓ)), problems) || throw(ArgumentError("every problem of a batch needs a non-empty parameter block"))
+        new(collect(DeviceLogDensity, problems), Int(K))
+    end
+end
+const AnyProblemBatch = Union{ProblemBatch,RaggedProblemBatch}
+family(b::AnyProblemBatch) = family(first(b.problems))
+params(b::AnyProblemBatch) = reduce(vcat, params.(b.problems))
+LogDensityProblems.dimension(b::AnyProblemBatch) = LogDensityProblems.dimension(first(b.problems))
+"Offsets of the blocks of a ragged batch in `params(b)`, [P + 1] (block p is params(b)[offsets[p]+1:offsets[p+1]])."
+block_offsets(b::RaggedProblemBatch) = Csize_t.(cumsum(vcat(0, length.(params.(b.problems)))))
 params(ℓ::DiagNormal) = vcat(ℓ.μ, 1 ./ ℓ.σ²)
 params(ℓ::LogisticRegression) = vcat(Float64(size(ℓ.X, 1)), vec(permutedims(ℓ.X)), ℓ.y)   # [N, X row-major, y]
 LogDensityProblems.capabilities(::Type{<:DeviceLogDensity}) = LogDensityProblems.LogDensityOrder{1}()
@@ -205,7 +225,10 @@ function _initialize(seed, ℓ::DeviceLogDensity, chains, initialization, algori
     h = Handle(Config(device, family(ℓ), D, chains, chain_offset, seed, algorithm.max_depth, 0,
                       algorithm.min_Δ, 0, 0))
     p = params(ℓ)
-    if ℓ isa ProblemBatch
+    if ℓ isa RaggedProblemBatch
+        _ck(h, ccall((:dhmc_set_problems_ragged, LIB), Cint, (Ptr{Cvoid}, Ptr{Float64}, Ptr{Csize_t}, Int64, Int64),
+                     h.ptr, p, block_offsets(ℓ), length(ℓ.problems), ℓ.K))
+    elseif ℓ isa ProblemBatch
         _ck(h, ccall((:dhmc_set_problems, LIB), Cint, (Ptr{Cvoid}, Ptr{Float64}, Csize_t, Int64, Int64),
                      h.ptr, p, length(p) ÷ length(ℓ.problems), length(ℓ.problems), ℓ.K))
     else
@@ -286,11 +309,14 @@ function mcmc_with_warmup(seed::Integer, ℓ::DeviceLogDensity, N::Integer; kwar
     [(; r.inference[k]..., κ = κ[k], ϵ = ϵ[k]) for k in eachindex(r.inference)]
 end
 
-# ---- problem batches: P posteriors, K chains each, one handle (dhmc_set_problems) ----------------------------
-"The results of P problems on one handle: element p is the vector of its K chains' NamedTuples (as `mcmc_with_warmup`)."
+# ---- problem batches: P posteriors, K chains each, one handle (dhmc_set_problems, _ragged) ----------------------------
+"""The results of P problems on one handle: element p is the vector of its K chains' NamedTuples (as `mcmc_with_warmup`).
+Problems whose parameter blocks differ in length (logistic regressions with different numbers of observations) form a
+RaggedProblemBatch, others a ProblemBatch."""
 function mcmc_with_warmup(seed::Integer, problems::AbstractVector{<:DeviceLogDensity}, N::Integer; chains_per_problem::Integer,
                           kwargs...)
-    b = ProblemBatch(problems, chains_per_problem)
+    ragged = !isempty(problems) && any(ℓ -> length(params(ℓ)) != length(params(first(problems))), problems)
+    b = ragged ? RaggedProblemBatch(problems, chains_per_problem) : ProblemBatch(problems, chains_per_problem)
     r = mcmc_with_warmup(seed, b, N; chains = length(problems) * b.K, kwargs...)
     [r[(p - 1) * b.K + 1:p * b.K] for p in eachindex(problems)]
 end
