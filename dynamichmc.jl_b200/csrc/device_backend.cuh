@@ -21,6 +21,8 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <type_traits>
+
 #include "../../include/dhmc_models.h"
 #include "nuts_machine.cuh"
 
@@ -581,6 +583,24 @@ struct DeviceBackend {
   const double* mparams;
   int n_slots;
 
+  // Per-element values that stay the same for the whole run of a chain and are cheap to recompute: the element index
+  // tid + e·T (and the lane-derived offsets of the reductions), the 1/√M⁻¹ of the momentum draw, the model's
+  // parameters.  Left alone, the compiler hoists them out of the transition and leaf loops and keeps them live across
+  // the whole tree build, where they crowd the state vectors (q, p, ∇ℓ, M⁻¹, ρ) out of the register budget into local
+  // memory.  pin() passes its input through an empty volatile asm, so that what is computed from it stays inside the
+  // loop that uses it.  With one element per thread the registers suffice and the recomputation would only cost time,
+  // so pin() is the identity there; packed chain groups keep their own register allocation (their time goes to the
+  // cooperative likelihood rounds).
+  static constexpr bool kPinInvariants = EPL >= 2 && PACK == 1;
+  template <class V> __device__ __forceinline__ static V pin(V v) {
+    if constexpr (kPinInvariants) {
+      if constexpr (std::is_pointer_v<V>) asm volatile("" : "+l"(v));
+      else if constexpr (std::is_same_v<V, double>) asm volatile("" : "+d"(v));
+      else asm volatile("" : "+r"(v));
+    }
+    return v;
+  }
+
   __device__ __forceinline__ bool valid(int e) const { return tid + e * T < D; }
   // slot base addresses are tabulated once per CTA in shared memory: one LDS.64 instead of a
   // 64-bit select + multiply-add at every access
@@ -729,7 +749,9 @@ struct DeviceBackend {
     if (lane == 0) ctl[j] = e;
     __syncwarp();
   }
-  __device__ __forceinline__ Entry get_entry(int j) const { return ctl[j]; }
+  // stack entries: the register-tight kernels read an entry's fields from shared memory where they are used, instead
+  // of holding a copy of all of them across merge_check
+  __device__ __forceinline__ std::conditional_t<kPinInvariants, const Entry&, Entry> get_entry(int j) const { return ctl[j]; }
 
   // all threads of the chain: the warp, or the CTA
   __device__ __forceinline__ void group_sync() const {
@@ -826,14 +848,14 @@ struct DeviceBackend {
         const double recv = __shfl_xor_sync(0xffffffffu, odd ? z0 : z1, 1);
         const double ze = odd ? recv : z0;        // element tid + e*T
         const double zo = odd ? z1 : recv;        // element tid + (e+1)*T
-        p[e] = (tid + e * T < D) ? dm_sqrt(1.0 / minv[e]) * ze : 0.0;
-        p[e + 1] = (tid + (e + 1) * T < D) ? dm_sqrt(1.0 / minv[e + 1]) * zo : 0.0;
+        p[e] = (tid + e * T < D) ? dm_sqrt(1.0 / pin(minv[e])) * ze : 0.0;
+        p[e + 1] = (tid + (e + 1) * T < D) ? dm_sqrt(1.0 / pin(minv[e + 1])) * zo : 0.0;
       }
     } else {
 #pragma unroll
       for (int e = 0; e < EPL; ++e) {
         const int i = tid + e * T;
-        p[e] = i < D ? dm_sqrt(1.0 / minv[e]) * dm_normal_elem(key, stream, t, (uint32_t)i) : 0.0;
+        p[e] = i < D ? dm_sqrt(1.0 / pin(minv[e])) * dm_normal_elem(key, stream, t, (uint32_t)i) : 0.0;
       }
     }
   }
@@ -1191,6 +1213,7 @@ struct DeviceBackend {
 
   // leapfrog(H, z, ϵ) — hamiltonian.jl:273-282, then logdensity(H, z′).
   __device__ __forceinline__ double leapfrog(double eps, int* flags) {
+    tid = pin(tid); lane = pin(lane); warp = pin(warp); mparams = pin(mparams);
     const double h = eps / 2;
     double qbad = 0.0;
     if constexpr (DENSE) {

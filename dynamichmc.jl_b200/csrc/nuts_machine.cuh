@@ -306,7 +306,7 @@ struct NutsMachine {
           while (!((k >> c) & 1u)) ++c;                   // ctz(k): merges after this leaf
 #endif
           for (int j = 0; j < c; ++j) {
-            const Entry E = b.get_entry(--sp);
+            const Entry& E = b.get_entry(--sp);
             const bool turning = b.merge_check(E.sfirst, E.slast, E.srho, L_sfirst, L_leaf);
             // v = combine_visited_statistics(v₋, v₊) precedes the checks, trees.jl:249
             // (ω of the merged tree is computed alongside: two independent logaddexp,
@@ -340,7 +340,7 @@ struct NutsMachine {
           // unwind: every pending ancestor combines its finished left half with
           // the invalid right half's v and passes the InvalidTree up (trees.jl:248-250)
           while (sp > 0) {
-            const Entry E = b.get_entry(--sp);
+            const Entry& E = b.get_entry(--sp);
             vacc_log = dm_logaddexp(E.vlog, vacc_log);
             vacc_steps = E.vsteps + vacc_steps;
           }
