@@ -204,6 +204,17 @@ inline bool dense_factor(const vec& Minv, int D, vec& W) {
   return cholesky_lower(M, D, W);
 }
 
+// The last dense factorisation of this thread, or one the caller supplied (orc_seed_dense_factor): every oracle call that
+// takes a Symmetric M⁻¹ builds its kinetic energy anew, and dense_factor is O(D³) (11 s at D = 2049), so a call whose M⁻¹
+// equals the cached one bit for bit reuses its W.  dense_factor is deterministic, so the cache changes no result.
+struct DenseFactorCache {
+  vec minv, w;
+};
+inline DenseFactorCache& dense_factor_cache() {
+  static thread_local DenseFactorCache c;
+  return c;
+}
+
 // GaussianKineticEnergy — src/hamiltonian.jl:56-87: Diagonal M⁻¹ (:80, :87) or dense
 // Symmetric M⁻¹ (:73).
 struct KineticEnergy {
@@ -219,7 +230,10 @@ struct KineticEnergy {
     KineticEnergy k(1);
     k.dense = true; k.D = D_; k.minv = M;
     if ((int)M.size() != D_ * D_) throw ArgumentError("checksquare(M⁻¹)");
+    DenseFactorCache& c = dense_factor_cache();
+    if (c.minv == M) { k.w = c.w; return k; }
     if (!dense_factor(M, D_, k.w)) throw DynamicHMCError("PosDefException: M⁻¹ is not positive definite");
+    c.minv = M; c.w = k.w;
     return k;
   }
   int size() const { return D; }                                     // :96
@@ -900,12 +914,12 @@ inline ChainOutput mcmc(Sampler& S, int N, WarmupState& st) {
   return out;
 }
 
-// initialize_warmup_state — mcmc.jl:129-132 (strict evaluation)
-inline WarmupState initialize_warmup_state(const Sampler& S, const vec* q, const vec* minv, const double* eps) {
+// initialize_warmup_state — mcmc.jl:129-132 (strict evaluation).  `dense`: minv is a Symmetric M⁻¹ [D*D] (the caller says so:
+// at D = 1 the two kinds have the same length)
+inline WarmupState initialize_warmup_state(const Sampler& S, const vec* q, const vec* minv, const double* eps,
+                                           bool dense = false) {
   vec q0 = q ? *q : random_position(S.key, S.l.D);
-  KineticEnergy k = !minv ? KineticEnergy(S.l.D)
-                    : ((int)minv->size() == S.l.D * S.l.D && S.l.D > 1 ? KineticEnergy::Dense(*minv, S.l.D)
-                                                                      : KineticEnergy(*minv));
+  KineticEnergy k = !minv ? KineticEnergy(S.l.D) : dense ? KineticEnergy::Dense(*minv, S.l.D) : KineticEnergy(*minv);
   return WarmupState{evaluate_l(S.l, q0, true), k, eps ? *eps : 0.0, eps != nullptr};
 }
 
@@ -913,9 +927,9 @@ inline WarmupState initialize_warmup_state(const Sampler& S, const vec* q, const
 struct McmcResult { ChainOutput inference; WarmupState final_state; std::vector<ChainOutput> warmup; };
 inline McmcResult mcmc_with_warmup(Sampler& S, int N, const std::vector<Stage>& stages,
                                    const vec* q = nullptr, const vec* minv = nullptr,
-                                   const double* eps = nullptr) {
+                                   const double* eps = nullptr, bool dense_minv = false) {
   S.alg.check();
-  WarmupState st = initialize_warmup_state(S, q, minv, eps);
+  WarmupState st = initialize_warmup_state(S, q, minv, eps, dense_minv);
   std::vector<ChainOutput> wu;
   for (const Stage& s : stages) {                       // _warmup fold, mcmc.jl:450-457
     if (s.kind == STAGE_NOTHING) { wu.push_back({}); continue; }   // :99-101

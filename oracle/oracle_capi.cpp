@@ -63,6 +63,13 @@ int orc_dense_factor(int D, const double* minv, double* W) {
   std::memcpy(W, w.data(), sizeof(double) * (size_t)D * D);
   return 0;
 }
+// W of M⁻¹ known to the caller (e.g. assembled from the dense_factor of the blocks of a block-diagonal M⁻¹): later calls
+// with this M⁻¹ use it instead of factorising
+void orc_seed_dense_factor(int D, const double* minv, const double* W) {
+  DenseFactorCache& c = dense_factor_cache();
+  c.minv.assign(minv, minv + (size_t)D * D);
+  c.w.assign(W, W + (size_t)D * D);
+}
 void orc_rand_p(uint64_t seed, uint64_t chain, uint32_t stream, uint32_t t, int D, const double* minv, double* out) {
   vec p = rand_p(dm_make_key(seed, chain), stream, t, make_k(minv, D));
   std::memcpy(out, p.data(), sizeof(double) * D);
@@ -334,7 +341,7 @@ int orc_mcmc_with_warmup(int family, int D, const double* params, int T, int max
     auto stages = make_stages(n_stages, kind, stN, metric, da_on, da4, search3);
     vec qv, mv; if (q0) qv.assign(q0, q0 + D);
     if (minv0) mv.assign(minv0, minv0 + (g_dense ? (size_t)D * D : (size_t)D));
-    auto r = mcmc_with_warmup(S, N, stages, q0 ? &qv : nullptr, minv0 ? &mv : nullptr, eps0);
+    auto r = mcmc_with_warmup(S, N, stages, q0 ? &qv : nullptr, minv0 ? &mv : nullptr, eps0, g_dense != 0);
     for (int i = 0; i < N; ++i) {
       if (posterior) std::memcpy(posterior + (size_t)i * D, r.inference.posterior[i].data(), sizeof(double) * D);
       if (stats) stats[i] = r.inference.stats[i];

@@ -154,6 +154,15 @@ def dense_factor(minv):
     return W
 
 
+def seed_dense_factor(minv, W):
+    """Let the following calls of this thread that take exactly this Symmetric M⁻¹ use W = cholesky(inv(M⁻¹)).L instead of
+    factorising M⁻¹ (O(D³)) themselves.  W must be what dense_factor(minv) returns."""
+    minv, W = _d(minv), _d(W)
+    D = minv.shape[0]
+    assert minv.shape == W.shape == (D, D)
+    lib().orc_seed_dense_factor(C.c_int(D), _p(minv), _p(W))
+
+
 def rand_p(seed, chain, stream, t, minv):
     D = np.asarray(minv).shape[0]
     out = np.empty(D)
