@@ -220,11 +220,12 @@ __global__ void k_tree_summary(const dhmc_tree_stats* stats, int N, int B, unsig
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
   for (int c = warp; c < B; c += nwarps) {
     const dhmc_tree_stats* s = stats + (size_t)c * N;
+    const double pi0 = s[0].pi;   // the mean is taken as π₀ + mean(π − π₀): a chain of constant π gets var = 0 exactly
     double a = 0.0, sp = 0.0, sd2 = 0.0;
     unsigned long long st = 0;
     for (int n = lane; n < N; n += 32) {
       const dhmc_tree_stats r = s[n];
-      a += r.acceptance_rate; st += (unsigned long long)r.steps; sp += r.pi;
+      a += r.acceptance_rate; st += (unsigned long long)r.steps; sp += r.pi - pi0;
       if (n + 1 < N) { const double d = s[n + 1].pi - r.pi; sd2 += d * d; }
       atomicAdd(depth_counts + (r.depth < 32 ? r.depth : 32), 1ull);
       const int k = (r.left == 1 && r.right == 0) ? 0 : (r.left == r.right ? 1 : 2);
@@ -234,7 +235,7 @@ __global__ void k_tree_summary(const dhmc_tree_stats* stats, int N, int B, unsig
       a += __shfl_xor_sync(0xffffffffu, a, o); sp += __shfl_xor_sync(0xffffffffu, sp, o);
       sd2 += __shfl_xor_sync(0xffffffffu, sd2, o); st += __shfl_xor_sync(0xffffffffu, st, o);
     }
-    const double mean = sp / N;
+    const double mean = pi0 + sp / N;
     double ss = 0.0;
     for (int n = lane; n < N; n += 32) { const double d = s[n].pi - mean; ss += d * d; }
     for (int o = 16; o; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
@@ -253,6 +254,14 @@ __global__ void k_tree_summary(const dhmc_tree_stats* stats, int N, int B, unsig
 //   sequence: a shift that keeps the variance of the means free of cancellation).  The host finishes R̂ and the Geyer sum.
 // Chain groups: local chain c belongs to group (off + c) / K — the problems of a batch; K = 0: one group of all chains.
 __device__ __forceinline__ int ess_group(long c, long long K, long long off) { return K ? (int)((off + c) / K) : 0; }
+// mean of one sequence (stride D) as x₀ + mean(x − x₀): a constant sequence gets its value exactly, so its centred draws,
+// W and (for equal constants) the variance of the means are exact zeros
+__device__ __forceinline__ double seq_mean(const double* x, int n, int D) {
+  const double x0 = x[0];
+  double s = 0.0;
+  for (int i = 0; i < n; ++i) s += x[(size_t)i * D] - x0;
+  return x0 + s / n;
+}
 __global__ void k_pilot_mean(const double* draws, int n, int N, int D, int B, long long K, long long off, int P, double* pilot) {
   const long t = (long)blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= (long)P * D) return;
@@ -260,9 +269,7 @@ __global__ void k_pilot_mean(const double* draws, int n, int N, int D, int B, lo
   const long long first = (long long)g * K - off;
   const long c0 = (K && first > 0) ? (long)first : 0;                            // the group's first local chain
   if (c0 >= B || ess_group(c0, K, off) != g) return;                            // no local chain: the host reports NaN
-  double s = 0.0;
-  for (int i = 0; i < n; ++i) s += draws[((size_t)c0 * N + i) * D + d];
-  pilot[t] = s / n;
+  pilot[t] = seq_mean(draws + (size_t)c0 * N * D + d, n, D);
 }
 __global__ void k_ess_rhat(const double* draws, int N, int n, int D, int B, long long K, long long off, int L, const double* pilot,
                            double* acc) {
@@ -275,9 +282,7 @@ __global__ void k_ess_rhat(const double* draws, int N, int n, int D, int B, long
     const int d = (int)(w % tiles) * 32 + lane;
     if (d >= D) continue;
     const double* x = draws + ((size_t)(seq >> 1) * N + (size_t)(seq & 1) * n) * D + d;
-    double mu = 0.0;
-    for (int i = 0; i < n; ++i) mu += x[(size_t)i * D];
-    mu /= n;
+    const double mu = seq_mean(x, n, D);
     const size_t gd = (size_t)ess_group(seq >> 1, K, off) * D + d;
     double* a = acc + gd * (L + 3);
     const double dm = mu - pilot[gd];
@@ -1466,7 +1471,9 @@ static int ess_rhat_groups(dhmc_handle* h, const double* draws_dev, int32_t N, i
       const double var_means = m > 1 ? (a[1] - a[0] * a[0] / m) / (m - 1.0) : 0.0;
       const double var_plus = mean_var * (dn - 1.0) / dn + var_means;        // (n−1)/n·W + B/n
       if (rhat) rhat[o] = std::sqrt(var_plus / mean_var);
-      if (ess) {
+      if (ess && !(var_plus > 0.0)) {
+        ess[o] = dm_nan();   // every sequence constant at one value: ρ̂ is 0/0 (MCMCDiagnosticTools returns NaN too)
+      } else if (ess) {
         // Geyer's initial monotone sequence on ρ̂_t = 1 − (W − mean acov_t) / var⁺, pairs (ρ̂_2k + ρ̂_2k+1)
         double tau = 0.0, prev = 1e300;
         for (int t = 0; t + 1 <= L; t += 2) {
@@ -1511,21 +1518,24 @@ int dhmc_acceptance_quantiles_dev(dhmc_handle* h, const dhmc_tree_stats* stats_d
   cudaFree(d_hist);
   if (e != cudaSuccess) { h->err = cudaGetErrorString(e); return DHMC_ECUDA; }
   const unsigned long long tot = n - hist[BINS];
+  // order statistic j (0-based) of the non-NaN rates, placed by its rank among the records of its bin: strictly inside
+  // the bin, so less than one bin width from the true value
+  auto order_stat = [&](unsigned long long j) {
+    unsigned long long cum = 0;
+    for (int b = 0; b < BINS; ++b) {
+      if (j < cum + hist[b]) return ((double)b + ((double)(j - cum) + 0.5) / (double)hist[b]) / BINS;
+      cum += hist[b];
+    }
+    return 1.0;
+  };
   for (int k = 0; k < nprobs; ++k) {
     if (!(probs[k] >= 0.0 && probs[k] <= 1.0)) { h->err = "0 ≤ p ≤ 1"; return DHMC_EARG; }
     if (tot == 0) { out[k] = dm_nan(); continue; }
-    const double target = probs[k] * (double)(tot - 1);             // Julia's quantile (type 7): position in the sorted sample
-    unsigned long long cum = 0;
-    double q = 1.0;
-    for (int b = 0; b < BINS; ++b) {
-      if ((double)(cum + hist[b]) > target) {                       // the order statistic lies in bin b: interpolate inside it
-        const double frac = hist[b] ? (target - (double)cum + 0.5) / (double)hist[b] : 0.5;
-        q = ((double)b + std::min(1.0, std::max(0.0, frac))) / BINS;
-        break;
-      }
-      cum += hist[b];
-    }
-    out[k] = q;
+    // Julia's quantile (type 7): x₍ⱼ₎ + γ (x₍ⱼ₊₁₎ − x₍ⱼ₎) at position p (n − 1) = j + γ of the sorted sample
+    const double pos = probs[k] * (double)(tot - 1);
+    const unsigned long long j = (unsigned long long)pos;
+    const double gamma = pos - (double)j, lo = order_stat(j);
+    out[k] = gamma > 0.0 ? lo + gamma * (order_stat(j + 1) - lo) : lo;
   }
   return DHMC_OK;
 }

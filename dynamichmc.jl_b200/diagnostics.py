@@ -9,9 +9,13 @@ ACCEPTANCE_QUANTILES = [0.05, 0.25, 0.5, 0.75, 0.95]      # diagnostics.jl:35
 
 
 def EBFMI(tree_statistics):
-    """diagnostics.jl:29-32: mean(abs2, diff(πs)) / var(πs) for one chain's statistics."""
+    """diagnostics.jl:29-32: mean(abs2, diff(πs)) / var(πs) for one chain's statistics.  The variance is taken of
+    πs − π₁, so a constant π gives 0 / 0 = NaN (as the device reduction does), not 0 over a rounding residue."""
     pis = np.asarray(tree_statistics["pi"], float)
-    return float(np.mean(np.diff(pis) ** 2) / np.var(pis, ddof=1))
+    if pis.size < 2:
+        return float("nan")
+    with np.errstate(invalid="ignore", divide="ignore"):
+        return float(np.mean(np.diff(pis) ** 2) / np.var(pis - pis[0], ddof=1))
 
 
 def count_terminations(tree_statistics):
@@ -154,7 +158,9 @@ def ess_rhat(draws, max_lag=0):
     Every chain is split in two halves (m = 2·chains sequences of n = N // 2 draws); W = mean within-sequence variance,
     var⁺ = (n−1)/n·W + var(sequence means); ρ̂_t = 1 − (W − mean_c acov_c(t)) / var⁺ with the biased autocovariance;
     τ = −1 + 2 Σ (ρ̂_2k + ρ̂_2k+1) over Geyer's initial monotone sequence; ESS = m·n / τ.  The quantities the reference's
-    correctness tests take from MCMCDiagnosticTools.ess_rhat (test/sample-correctness_utilities.jl:40-43)."""
+    correctness tests take from MCMCDiagnosticTools.ess_rhat (test/sample-correctness_utilities.jl:40-43).  A sequence's
+    mean is x₁ + mean(x − x₁), so constant sequences centre to exact zeros; a parameter whose sequences are all constant
+    at one value (var⁺ = 0) gets R̂ = ESS = NaN, as in MCMCDiagnosticTools."""
     x = np.asarray(draws, float)
     K, N, D = x.shape
     n = N // 2
@@ -162,15 +168,16 @@ def ess_rhat(draws, max_lag=0):
     L = max(1, min(L, n - 2))
     seq = np.stack([x[:, :n], x[:, n:2 * n]], axis=1).reshape(2 * K, n, D)     # sequence 2c = first half of chain c, 2c+1 = second
     m = 2 * K
-    mu = seq.mean(axis=1)                                      # [m, D]
+    mu = seq[:, 0] + (seq - seq[:, :1]).mean(axis=1)          # [m, D]
     xc = seq - mu[:, None, :]
     acov = np.stack([(xc[:, : n - t] * xc[:, t:]).sum(axis=1) / n for t in range(L + 1)])   # [L+1, m, D]
     mean_var = acov[0].mean(axis=0) * n / (n - 1.0)
-    var_plus = mean_var * (n - 1.0) / n + (mu.var(axis=0, ddof=1) if m > 1 else 0.0)
-    rhat = np.sqrt(var_plus / mean_var)
-    rho = 1.0 - (mean_var[None] - acov.mean(axis=1)) / var_plus[None]                      # [L+1, D]
-    ess = np.empty(D)
-    for d in range(D):
+    var_plus = mean_var * (n - 1.0) / n + ((mu - mu[0]).var(axis=0, ddof=1) if m > 1 else 0.0)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        rhat = np.sqrt(var_plus / mean_var)
+        rho = 1.0 - (mean_var[None] - acov.mean(axis=1)) / var_plus[None]                  # [L+1, D]
+    ess = np.full(D, np.nan)
+    for d in np.flatnonzero(var_plus > 0):
         tau, prev = 0.0, np.inf
         for t in range(0, L, 2):
             pair = rho[t, d] + rho[t + 1, d]

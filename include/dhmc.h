@@ -212,7 +212,9 @@ int dhmc_mcmc_dev(dhmc_handle* h, int32_t N, double* posterior, dhmc_tree_stats*
 /* Diagnostics.summarize_tree_statistics / EBFMI (diagnostics.jl:29-32, 65-106) reduced on the
  * GPU over stats_dev [N,B] (DEVICE pointer, e.g. the buffer given to dhmc_mcmc_dev): pooled
  * depth counts [33], termination counts [max_depth, divergence, turning], Σ acceptance rate,
- * Σ steps (host outputs, may be NULL) and the per-chain EBFMI [B] (host, may be NULL). */
+ * Σ steps (host outputs, may be NULL) and the per-chain EBFMI [B] (host, may be NULL).  EBFMI is NaN for N = 1 and
+ * for a chain whose π is constant (0 / 0: π is centred on its first value, so a constant π has variance exactly 0; Julia's
+ * EBFMI returns 0 there when its mean of the constant rounds away from it). */
 int dhmc_tree_summary_dev(dhmc_handle* h, const dhmc_tree_stats* stats_dev, int32_t N,
                           int64_t* depth_counts, int64_t* termination_counts,
                           double* acceptance_sum, int64_t* steps_sum, double* ebfmi);
@@ -220,7 +222,8 @@ int dhmc_tree_summary_dev(dhmc_handle* h, const dhmc_tree_stats* stats_dev, int3
 /* Cross-chain convergence diagnostics reduced on the GPU over device-resident draws [D, N, B] (the posterior buffer of
  * dhmc_mcmc_dev): per parameter the split-R̂ and the effective sample size of the pooled sequences (every chain split in two
  * halves; autocorrelations up to max_lag ≤ N/2 − 2, 0 = 64; Geyer's initial monotone sequence) — what the reference's
- * correctness tests compute with MCMCDiagnosticTools.ess_rhat (test/sample-correctness_utilities.jl:40-43).
+ * correctness tests compute with MCMCDiagnosticTools.ess_rhat (test/sample-correctness_utilities.jl:40-43).  A parameter
+ * whose sequences are all constant at one value (var⁺ = 0) gets ESS = NaN and R̂ = NaN, as in MCMCDiagnosticTools.
  * rhat, ess: host [D], either may be NULL. */
 int dhmc_ess_rhat_dev(dhmc_handle* h, const double* draws_dev, int32_t N, int32_t max_lag, double* rhat, double* ess);
 /* The same per (problem, parameter) of a problem batch, over each problem's local chains (dhmc_ess_rhat_dev pools all
@@ -229,7 +232,9 @@ int dhmc_ess_rhat_dev(dhmc_handle* h, const double* draws_dev, int32_t N, int32_
 int dhmc_ess_rhat_problems_dev(dhmc_handle* h, const double* draws_dev, int32_t N, int32_t max_lag, double* rhat,
                                double* ess);
 /* Quantiles of the acceptance rates (Diagnostics.summarize_tree_statistics: a_quantiles at 0.05 … 0.95,
- * diagnostics.jl:35,100-106) of a device statistics buffer [N, B], from a 4096-bin histogram (resolution 2.4e-4). */
+ * diagnostics.jl:35,100-106) of a device statistics buffer [N, B], from a 4096-bin histogram: the two order statistics
+ * Julia's type-7 quantile interpolates between are each placed inside their bin, so every quantile is within 1/4096
+ * (2.4e-4) of the type-7 quantile of the records whose rate is not NaN (those are left out; none left: NaN). */
 int dhmc_acceptance_quantiles_dev(dhmc_handle* h, const dhmc_tree_stats* stats_dev, int32_t N, const double* probs,
                                   int32_t nprobs, double* out);
 

@@ -32,10 +32,30 @@ STD, DIAG, FUNNEL, LOGISTIC, USER = 0, 1, 2, 3, 4      # include/dhmc.h DHMC_FAM
 FAMILY_NAMES = {STD: "std", DIAG: "diag", FUNNEL: "funnel", LOGISTIC: "logistic", USER: "rosenbrock"}
 TEMPLATE_KERNELS = ("k_nuts", "k_search", "k_leapfrog", "k_eval", "k_phase")
 HEAVY = ("k_nuts", "k_search")
-# the host's utility kernels (dhmc_b200.cu): not templates of a layout, checked by the suite's other tests
-UTILITY_KERNELS = ("k_dense_factor", "k_cov_finish", "k_cov_pool", "k_pad_metric", "k_pad_rows", "k_transpose",
-                   "k_tree_summary", "k_pilot_mean", "k_ess_rhat", "k_acceptance_hist", "k_broadcast", "k_broadcast_mat",
-                   "k_fill")
+# the host's utility kernels (dhmc_b200.cu), not templates of a layout: {kernel: the test (file::name) whose results
+# depend on it, against the oracle or an exact reference}
+UTILITY_KERNELS = {
+    # M⁻¹ set per chain (Symmetric phase) and the factor of a shared one, bit-equal to the oracle's trees
+    "k_dense_factor": "test_kernel_coverage.py::test_case_matches_oracle",
+    # the window estimate of a Symmetric / pooled Symmetric stage against the exact covariance of the window
+    "k_cov_finish": "test_utility_kernels.py::test_window_metric_is_the_regularized_covariance_of_the_window",
+    "k_cov_pool": "test_utility_kernels.py::test_window_metric_is_the_regularized_covariance_of_the_window",
+    # the packed logistic cases (8 chains per CTA): padded M⁻¹ blocks (dense phase) and padded rows of X
+    "k_pad_metric": "test_kernel_coverage.py::test_case_matches_oracle",
+    "k_pad_rows": "test_kernel_coverage.py::test_case_matches_oracle",
+    # Xᵀ of every logistic case
+    "k_transpose": "test_kernel_coverage.py::test_case_matches_oracle",
+    "k_tree_summary": "test_utility_kernels.py::test_tree_summary_matches_the_exact_reference",
+    "k_pilot_mean": "test_utility_kernels.py::test_ess_rhat_matches_the_exact_reference",
+    "k_ess_rhat": "test_utility_kernels.py::test_ess_rhat_matches_the_exact_reference",
+    "k_acceptance_hist": "test_utility_kernels.py::test_acceptance_quantiles_within_one_bin_of_type7",
+    # one diagonal M⁻¹ [D] broadcast to every chain, then trees against the oracle
+    "k_broadcast": "test_gpu_parity.py::test_one_dimensional_problem",
+    # one Symmetric M⁻¹ [D, D] broadcast to every chain (the cases above dim 256)
+    "k_broadcast_mat": "test_kernel_coverage.py::test_case_matches_oracle",
+    # a scalar step size filled into every chain, then trees against the oracle
+    "k_fill": "test_gpu_parity.py::test_one_dimensional_problem",
+}
 # shipped instantiations no handle can launch: {name: reason}
 UNREACHABLE = {}
 
@@ -224,6 +244,21 @@ def test_every_shipped_instantiation_is_claimed_by_a_case(pkg):
     print(f"\n{len(every)} shipped template-kernel instantiations ({len(shipped['stock'])} in libdhmc_b200.so, "
           f"{len(shipped['rosenbrock'])} in the Rosenbrock library); {len(every & set(claimed))} launched by the "
           f"{len(CASES)} cases, {len(UNREACHABLE)} unreachable")
+
+
+def test_every_shipped_utility_kernel_names_an_existing_test(pkg):
+    """every non-template entry function of the libraries has an entry in UTILITY_KERNELS, and the test it names exists"""
+    for so in (os.path.join(CSRC, "libdhmc_b200.so"), pkg.compile_user_model(ROSENBROCK, deep=True)):
+        util = {n for n in _entry_functions(so) if "<" not in n}
+        missing = sorted(util - set(UTILITY_KERNELS))
+        assert not missing, f"{os.path.basename(so)}: utility kernel(s) without a test in UTILITY_KERNELS: {missing}"
+        assert not set(UTILITY_KERNELS) - util, f"UTILITY_KERNELS lists kernels that do not ship: {set(UTILITY_KERNELS) - util}"
+    for kernel, where in UTILITY_KERNELS.items():
+        fname, test = where.split("::")
+        path = os.path.join(ROOT, "tests", fname)
+        assert os.path.isfile(path), (kernel, where)
+        with open(path, encoding="utf-8") as f:
+            assert re.search(r"^def %s\(" % re.escape(test), f.read(), re.M), f"{kernel}: no test {where}"
 
 
 def test_layout_rules_agree_with_the_shipped_layouts(pkg):
