@@ -9,6 +9,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("DHMC_B200_LIB", os.path.join(_HERE, "csrc", "libdhmc_b200.so"))
 
 DHMC_OK, DHMC_EARG, DHMC_ENUMERIC, DHMC_ECUDA, DHMC_ENOMEM, DHMC_ENCCL = 0, 1, 2, 3, 4, 5
+DHMC_CHAIN_BAD_INITIAL, DHMC_CHAIN_NONFINITE_Q, DHMC_CHAIN_LEAPFROG_NONFINITE = 1, 4, 64   # per-chain status bits (include/dhmc.h)
 COMM_ID_BYTES = 128
 FAMILY_STD_NORMAL, FAMILY_DIAG_NORMAL, FAMILY_FUNNEL, FAMILY_LOGISTIC, FAMILY_USER = 0, 1, 2, 3, 4
 METRIC_NOTHING, METRIC_DIAGONAL, METRIC_SYMMETRIC, METRIC_SYMMETRIC_POOLED = 0, 1, 2, 3

@@ -36,7 +36,12 @@ class DynamicHMCError(Exception):
 
 
 class ArgumentError(ValueError):
-    """Julia's ArgumentError raised by @argcheck in the reference."""
+    """Julia's ArgumentError raised by @argcheck in the reference.  A per-chain one (leapfrog from a non-finite log
+    density, hamiltonian.jl:276) carries the chain status words in `debug_information`, as DynamicHMCError does."""
+
+    def __init__(self, message, **debug_information):
+        super().__init__(message)
+        self.debug_information = debug_information
 
 
 def _argcheck(cond, msg):
@@ -461,7 +466,14 @@ class Engine:
         if rc == L.DHMC_EARG:
             raise ArgumentError(msg)
         if rc == L.DHMC_ENUMERIC:
-            raise DynamicHMCError(msg, chain_status=self.chain_status())
+            st = self.chain_status()
+            # leapfrog's @argcheck isfinite(Q.ℓq) (hamiltonian.jl:276) is an ArgumentError in the reference; a chain whose
+            # strict initial evaluation failed, or that met a non-finite position first, has failed with DynamicHMCError
+            # before it got there
+            halted = (st & L.DHMC_CHAIN_LEAPFROG_NONFINITE) != 0
+            if np.any(halted & ((st & (L.DHMC_CHAIN_BAD_INITIAL | L.DHMC_CHAIN_NONFINITE_Q)) == 0)):
+                raise ArgumentError(msg, chain_status=st)
+            raise DynamicHMCError(msg, chain_status=st)
         raise RuntimeError(f"libdhmc_b200 error [{rc}]: {msg}")
 
     def close(self):

@@ -520,9 +520,23 @@ static int sync_and_check_status(dhmc_handle* h, int mask, const char* what) {
   const size_t B = (size_t)h->cfg.n_chains;
   std::vector<int> st(B);
   CK(cudaMemcpy(st.data(), h->status, sizeof(int) * B, cudaMemcpyDeviceToHost));
-  long bad = 0, first = -1;
-  for (size_t i = 0; i < B; ++i)
+  long bad = 0, first = -1, halted = 0, first_halted = -1;
+  for (size_t i = 0; i < B; ++i) {
     if (st[i] & mask) { if (first < 0) first = (long)i; ++bad; }
+    // a chain whose first failure is leapfrog's @argcheck (a strict evaluation or a non-finite position fails earlier)
+    if ((st[i] & mask & DHMC_CHAIN_LEAPFROG_NONFINITE) && !(st[i] & (DHMC_CHAIN_BAD_INITIAL | DHMC_CHAIN_NONFINITE_Q))) {
+      if (first_halted < 0) first_halted = (long)i;
+      ++halted;
+    }
+  }
+  if (halted) {      // the ArgumentError of hamiltonian.jl:276 is named first: the shims raise it for these chains
+    char buf[320];
+    std::snprintf(buf, sizeof buf,
+                  "Internal error: leapfrog called from non-finite log density: %ld chain(s) (first: local chain %ld, "
+                  "status 0x%x); %ld chain(s) failed in all (%s)", halted, first_halted, st[first_halted], bad, what);
+    h->err = buf;
+    return DHMC_ENUMERIC;
+  }
   if (bad) {
     char buf[256];
     std::snprintf(buf, sizeof buf, "%s: %ld chain(s) failed (first: local chain %ld, status 0x%x)",
@@ -1063,7 +1077,8 @@ int dhmc_leapfrog(dhmc_handle* h, int32_t n_steps, int32_t sign) {
   a.lf_steps = n_steps; a.lf_sign = sign;
   int rc = launch(h, K_LEAPFROG, a, 1);
   if (rc != DHMC_OK) return rc;
-  return sync_and_check_status(h, DHMC_CHAIN_NONFINITE_Q, "leapfrog: position vector has non-finite elements");
+  return sync_and_check_status(h, DHMC_CHAIN_NONFINITE_Q | DHMC_CHAIN_LEAPFROG_NONFINITE,
+                               "leapfrog: position vector has non-finite elements");
 }
 
 int dhmc_phase_logdensity(dhmc_handle* h, double* out) {
@@ -1278,7 +1293,8 @@ static int run_nuts(dhmc_handle* h, int N, const AdaptConfig& cfg, double lambda
   if (advance_t) h->t += (uint32_t)N;
   if (q_host) h->has_position = true;
   if (h->trace) std::fprintf(stderr, "[dhmc trace] host: before status check %.2f ms\n", tr_ms());
-  rc = sync_and_check_status(h, DHMC_CHAIN_NONFINITE_Q | DHMC_CHAIN_BAD_ACCEPTANCE | DHMC_CHAIN_BAD_STEPSIZE | (q_host ? DHMC_CHAIN_BAD_INITIAL : 0),
+  rc = sync_and_check_status(h, DHMC_CHAIN_NONFINITE_Q | DHMC_CHAIN_BAD_ACCEPTANCE | DHMC_CHAIN_BAD_STEPSIZE |
+                                    DHMC_CHAIN_LEAPFROG_NONFINITE | (q_host ? DHMC_CHAIN_BAD_INITIAL : 0),
                              q_host ? "invalid initial position, or non-finite position / acceptance rate / step size while sampling"
                                     : "sampling: non-finite position, acceptance rate or step size");
   if (h->trace) std::fprintf(stderr, "[dhmc trace] host: after status check %.2f ms\n", tr_ms());

@@ -263,12 +263,17 @@ __global__ void __launch_bounds__(32 * W * G, G > 1 ? 1 : min_ctas(W, EPL)) k_nu
     const double eps_next = m.run(a.t0, a.N, a.eps[c], a.cfg, a.p_override,
                                   a.dir_override ? a.dir_override + c : nullptr, sink);
     const size_t base = (size_t)c * a.D;
-    store_vec(b, a.q, b.q, base, a.D);
-    store_vec(b, a.g, b.g, base, a.D);
-    if (a.cfg.metric == DHMC_METRIC_DIAGONAL) store_vec(b, a.minv, b.minv, base, a.D);
+    const bool halted = (m.status & DHMC_CHAIN_LEAPFROG_NONFINITE) != 0;   // the chain keeps the state the call found it in
+    if (!halted) {
+      store_vec(b, a.q, b.q, base, a.D);
+      store_vec(b, a.g, b.g, base, a.D);
+      if (a.cfg.metric == DHMC_METRIC_DIAGONAL) store_vec(b, a.minv, b.minv, base, a.D);
+    }
     if (b.tid == 0) {
-      a.lq[c] = b.lq;
-      a.eps[c] = eps_next;
+      if (!halted) {
+        a.lq[c] = b.lq;
+        a.eps[c] = eps_next;
+      }
       if (m.status) atomicOr(a.status + c, m.status);
       atomicAdd(a.total_steps, (unsigned long long)m.steps_out);
     }
@@ -318,14 +323,22 @@ __global__ void __launch_bounds__(32 * W, min_ctas(W, EPL)) k_leapfrog(const KAr
     load_chain(b, a, c, true);
     const double eps = a.lf_sign >= 0 ? a.eps[c] : -a.eps[c];
     int flags = 0;
-    for (int s = 0; s < a.lf_steps; ++s) (void)b.leapfrog(eps, &flags);
+    bool halted = false;
+    for (int s = 0; s < a.lf_steps; ++s) {
+      // @argcheck isfinite(Q.ℓq), hamiltonian.jl:276 (after a non-finite position the reference has raised already)
+      if (!dm_isfinite(b.lq) && !(flags & 1)) { halted = true; break; }
+      (void)b.leapfrog(eps, &flags);
+    }
     const size_t base = (size_t)c * a.D;
-    store_vec(b, a.q, b.q, base, a.D);
-    store_vec(b, a.p, b.p, base, a.D);
-    store_vec(b, a.g, b.g, base, a.D);
+    if (!halted) {                         // a halted chain keeps the state the call found it in
+      store_vec(b, a.q, b.q, base, a.D);
+      store_vec(b, a.p, b.p, base, a.D);
+      store_vec(b, a.g, b.g, base, a.D);
+    }
     if (b.tid == 0) {
-      a.lq[c] = b.lq;
+      if (!halted) a.lq[c] = b.lq;
       if (flags & 1) atomicOr(a.status + c, (int)DHMC_CHAIN_NONFINITE_Q);
+      if (halted) atomicOr(a.status + c, (int)DHMC_CHAIN_LEAPFROG_NONFINITE);
     }
     if (W > 1) __syncthreads();
   }

@@ -220,7 +220,9 @@ struct NutsMachine {
   }
 
   // One NUTS transition from the backend's current (q, ℓq, ∇ℓq).
-  // On return the backend's current point is the new position ζ.Q.
+  // On return the backend's current point is the new position ζ.Q — unless a leapfrog would have started from a
+  // non-finite ℓ: then DHMC_CHAIN_LEAPFROG_NONFINITE is set, *ts is not written and the backend's point is
+  // meaningless (the caller keeps the chain's stored state).
   DHMC_M void transition(uint32_t t_, double eps, const double* p_override,
                           const uint32_t* dir_override, dhmc_tree_stats* ts) {
     t = t_;
@@ -285,6 +287,10 @@ struct NutsMachine {
       int L_vsteps = 0, L_ifirst = 0, L_sfirst = -1, L_szq = -1, L_szg = -1;
       bool L_leaf = true;
       for (unsigned k = 1; k <= nleaves; ++k) {
+        if (!dm_isfinite(b.cur_lq())) {                   // @argcheck isfinite(Q.ℓq), hamiltonian.jl:276
+          status |= DHMC_CHAIN_LEAPFROG_NONFINITE;
+          break;
+        }
         int lf_flags = 0;
         const double Hn = b.leapfrog(eps_s, &lf_flags);   // move + logdensity(H, z′)
         if (lf_flags & 1) status |= DHMC_CHAIN_NONFINITE_Q;
@@ -371,6 +377,7 @@ struct NutsMachine {
           vacc_log = L_vlog; vacc_steps = L_vsteps;
         }
       }
+      if (status & DHMC_CHAIN_LEAPFROG_NONFINITE) return;   // the reference raises: no statistics, no new position
       // ---------------- back in sample_trajectory ----------------
       double om_top;
       b.logaddexp2(v_log, vacc_log, omega_top, L_omega, &v_log, &om_top);   // trees.jl:294, :310
@@ -457,6 +464,7 @@ struct NutsMachine {
       const double e = cfg.adapt ? dm_exp(S.da_logeps) : eps;   // current_ϵ :163
       dhmc_tree_stats ts;
       transition(t0 + (uint32_t)n, e, p_override, dir_override, &ts);
+      if (status & DHMC_CHAIN_LEAPFROG_NONFINITE) { steps_out = S.total_steps; return eps; }   // the chain stops here
       S.total_steps += ts.steps;
       sink(n, ts, e);
       if (cfg.adapt) {

@@ -46,7 +46,11 @@ enum {
   DHMC_CHAIN_NONFINITE_Q = 4,   /* evaluate_ℓ: non-finite position, hamiltonian.jl:203 */
   DHMC_CHAIN_BAD_ACCEPTANCE = 8, /* adapt_stepsize @argcheck 0 ≤ a ≤ 1, stepsize.jl:148 */
   DHMC_CHAIN_NOT_POSDEF = 16,    /* cholesky(inv(M⁻¹)) failed, hamiltonian.jl:73 (PosDefException) */
-  DHMC_CHAIN_BAD_STEPSIZE = 32   /* initial_adaptation_state @argcheck ϵ > 0, stepsize.jl:135 (chain left untouched) */
+  DHMC_CHAIN_BAD_STEPSIZE = 32,  /* initial_adaptation_state @argcheck ϵ > 0, stepsize.jl:135 (chain left untouched) */
+  DHMC_CHAIN_LEAPFROG_NONFINITE = 64 /* leapfrog @argcheck isfinite(Q.ℓq), hamiltonian.jl:276 ("leapfrog called from
+                                        non-finite log density"; the shims raise ArgumentError): a leapfrog would start
+                                        from ℓ = −∞, e.g. after ℓ(q₀) = −∞ or a non-divergent leaf at ℓ = −∞ (min_Δ = −Inf,
+                                        or π₀ = −∞ makes Δ NaN).  The chain stops and keeps the state the call found it in. */
 };
 
 /* log-density family ids: see include/dhmc_models.h */

@@ -78,6 +78,10 @@ DHMC_HD double dhmc_logit_eta(const double* xrow, const double* beta, int D) { r
  *   σ(η) = 1/(1+t) for η >= 0, t/(1+t) for η < 0   (no cancellation; one correctly rounded division) */
 DHMC_HD void dhmc_logit_finish(double y, double eta, double sp, double t, double* ll, double* resid) {
   *ll = y * eta - ((eta > 0.0 ? eta : 0.0) + sp);
+  /* η = ±∞ (the dot product overflowed): the formula gives ∞ − ∞ or 0·∞ = NaN, the limit is 0 for the outcome the sign
+   * predicts (y = 1 at +∞, y = 0 at −∞) and −∞ otherwise.  Finite η keep the formula's value bit for bit. */
+  if (eta == dm_inf()) *ll = y == 1.0 ? 0.0 : -dm_inf();
+  if (eta == -dm_inf()) *ll = y == 0.0 ? 0.0 : -dm_inf();
   const double u = 1.0 + t;
   const double s = (eta >= 0.0 ? 1.0 : t) / u;
   *resid = y - s;

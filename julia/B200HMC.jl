@@ -35,6 +35,7 @@ end
 @assert sizeof(TreeStatisticsNUTS) == 56
 
 const OK, EARG, ENUMERIC = 0, 1, 2
+const CHAIN_BAD_INITIAL, CHAIN_NONFINITE_Q, CHAIN_LEAPFROG_NONFINITE = Int32(1), Int32(4), Int32(64)   # per-chain status bits
 
 mutable struct Handle
     ptr::Ptr{Cvoid}
@@ -59,6 +60,11 @@ function _throw(rc, ptr, K)
     rc == EARG && throw(ArgumentError(msg))
     if rc == ENUMERIC
         status = ptr == C_NULL ? Int32[] : chain_status(ptr, K)
+        # leapfrog's @argcheck isfinite(Q.ℓq) (hamiltonian.jl:276) is an ArgumentError; a chain whose strict initial
+        # evaluation failed or that met a non-finite position first has failed with DynamicHMCError before it got there
+        halted = findall(s -> (s & CHAIN_LEAPFROG_NONFINITE) != 0 && (s & (CHAIN_BAD_INITIAL | CHAIN_NONFINITE_Q)) == 0,
+                         status)
+        isempty(halted) || throw(ArgumentError("$msg (chains $halted)"))
         throw(DynamicHMCError(msg, (; failed_chains = findall(!iszero, status), status)))
     end
     error("libdhmc_b200 error [$rc]: $msg")

@@ -162,3 +162,18 @@ def test_julia_shim_passes_the_chain_count_to_chain_status():
     for needle in ("dhmc_metric_is_dense", "dhmc_get_metric_dense", "Symmetric(M", "function mcmc_keep_warmup", "mcmc_steps(",
                    "function mcmc_next_step", "reporter"):
         assert needle in jl, needle
+
+
+def test_chain_status_bits_match_header(pkg):
+    """The status bits the Python and Julia shims map to exceptions are the header's."""
+    src = open(os.path.join(ROOT, "include", "dhmc.h")).read()
+    bits = {m.group(1): int(m.group(2)) for m in re.finditer(r"\b(DHMC_CHAIN_[A-Z_]+)\s*=\s*(\d+)", src)}
+    assert bits["DHMC_CHAIN_NONFINITE_Q"] == pkg._lib.DHMC_CHAIN_NONFINITE_Q
+    assert bits["DHMC_CHAIN_BAD_INITIAL"] == pkg._lib.DHMC_CHAIN_BAD_INITIAL
+    assert bits["DHMC_CHAIN_LEAPFROG_NONFINITE"] == pkg._lib.DHMC_CHAIN_LEAPFROG_NONFINITE
+    assert sorted(bits.values()) == [1 << i for i in range(len(bits))]      # distinct single bits
+    jl = open(os.path.join(ROOT, "julia", "B200HMC.jl")).read()
+    m = re.search(r"const CHAIN_BAD_INITIAL, CHAIN_NONFINITE_Q, CHAIN_LEAPFROG_NONFINITE = "
+                  r"Int32\((\d+)\), Int32\((\d+)\), Int32\((\d+)\)", jl)
+    assert m and tuple(int(g) for g in m.groups()) == (bits["DHMC_CHAIN_BAD_INITIAL"], bits["DHMC_CHAIN_NONFINITE_Q"],
+                                                        bits["DHMC_CHAIN_LEAPFROG_NONFINITE"])

@@ -30,6 +30,38 @@ def test_exp_log_accuracy(po):
     assert _max_ulp(po.math("cos2pi", u), [mp.cos(2 * mp.pi * mp.mpf(float(v))) for v in u]) < 3
 
 
+def test_exp_at_underflow_and_overflow(po):
+    """dm_exp where the funnel's exp(−v) and the logistic link leave the normal range.  On [−745.14, −708.4] the result
+    is subnormal (or rounds to 0), and the error is bounded in units of the subnormal spacing 2⁻¹⁰⁷⁴: below 1 everywhere
+    (one of the two neighbours of the true value), and within 0.5 + 2⁻⁷ below 2⁻¹⁰³⁰, where the polynomial's relative
+    error is worth less than 2⁻⁸ spacings — one rounding into the subnormal range, no double rounding.  Near
+    log(floatmax) = 709.7827… the result is within 1.5 ulp, and +Inf exactly where the true value rounds past floatmax."""
+    mp.mp.prec = 200
+    rng = np.random.default_rng(1)
+    sub = 2.0 ** -1074
+    x = np.concatenate([rng.uniform(-745.14, -708.4, 6000), rng.uniform(-745.14, -744.0, 1000),
+                        [-745.1332191019412, -745.13321910194122, -745.1332191019411, -708.3964185322641,
+                         -708.39641853226408, -744.44007192138126, -745.14]])
+    got = po.math("exp", x)
+    ref = [mp.exp(mp.mpf(float(v))) for v in x]
+    err = np.array([float(abs(mp.mpf(float(g)) - r) / sub) for g, r in zip(got, ref)])
+    deep = np.array([r < mp.mpf(2) ** -1030 for r in ref])
+    assert np.all(got >= 0)
+    assert err.max() < 1.0, x[np.argmax(err)]
+    assert deep.sum() > 2000 and err[deep].max() <= 0.5 + 2 ** -7, x[deep][np.argmax(err[deep])]
+    assert np.any(got == 0.0) and np.any(got == sub)        # the two ends: rounds to 0, to the smallest subnormal
+    fmax = np.finfo(np.float64).max
+    x = np.concatenate([rng.uniform(709.0, 709.782712893384, 3000), np.nextafter(709.782712893384, 0) - np.arange(50) * 1e-13,
+                        [709.782712893384, np.nextafter(709.782712893384, np.inf), 709.79]])
+    got = po.math("exp", x)
+    for g, v in zip(got, x):
+        ref = mp.exp(mp.mpf(float(v)))
+        if ref >= mp.mpf(fmax) + mp.mpf(2) ** 970:                # rounds to +Inf in binary64 (half an ulp of floatmax)
+            assert g == np.inf, v
+        else:
+            assert np.isfinite(g) and abs(mp.mpf(float(g)) - ref) / np.spacing(float(ref)) < 1.5, v
+
+
 def test_softplus_table_accuracy(po):
     """dm_softplus_neg(d) = log(1 + exp(-d)): table-driven, absolute error ~1e-16 (it is always
     added to max(a, b) inside logaddexp)."""

@@ -191,3 +191,71 @@ def test_hypothesis_single_transition(po, family, D, T, logeps, max_depth, seed,
                min_delta=min_delta, directions=dirs)
     _same_stats(o["stats"], h["tree_statistics"][0])
     assert np.array_equal(o["q"], h["q"]) and o["lq"] == h["lq"]
+
+
+# ---- leapfrog's @argcheck isfinite(Q.ℓq) (hamiltonian.jl:276): a leapfrog never starts from ℓ = −∞ ----
+LEAPFROG_NONFINITE = 64     # DHMC_CHAIN_LEAPFROG_NONFINITE, include/dhmc.h
+
+
+def _raises_leapfrog_argcheck(po, fn):
+    try:
+        fn()
+    except po.OracleError as e:
+        assert e.status == 1 and "leapfrog called from non-finite log density" in str(e), e
+        return True
+    return False
+
+
+def test_leapfrog_from_nonfinite_density_halts_the_chain(po):
+    """The two ways a tree reaches a leapfrog from ℓ = −∞, where the reference raises ArgumentError and the machine used
+    to go on with status 0: (1) min_Δ = −Inf: from q₀ = 1e153 the first leaf lands where q² overflows, ℓ = −∞ there, Δ = −∞
+    is not below min_Δ, so the leaf is not divergent and the next leapfrog starts from it; (2) a strict evaluation accepts
+    ℓ(q₀) = −∞ (q₀² overflows), and the first leapfrog starts from q₀.  The machine flags the chain and stops it, also when
+    the call asked for more transitions.  (That the chain then keeps its stored state is the kernels' part: k_nuts and
+    k_leapfrog do not write a halted chain back, which the GPU tests check.)"""
+    D = 4
+    params = np.concatenate([np.zeros(D), np.ones(D)])
+    for q, eps, min_delta in ((np.array([1e153, 0, 0, 0.]), 5.0, -np.inf), (np.array([2e154, 0, 0, 0.]), 0.5, -1000.0)):
+        po.evaluate_l(1, q, params, strict=True)            # accepted: ℓ(q₀) is finite, or −∞
+        assert _raises_leapfrog_argcheck(po, lambda: po.sample_tree(1, q, eps, 1, 0, 0, params=params, min_delta=min_delta))
+        for N in (1, 3):
+            h = hs.run(1, q, eps, 1, 0, N=N, params=params, min_delta=min_delta)
+            assert h["status"] == LEAPFROG_NONFINITE
+            assert np.all(h["tree_statistics"]["steps"] == 0)     # it halts in its first transition: nothing recorded
+
+
+def test_near_overflow_starts_match_oracle():
+    """Random starts near overflow that a strict evaluation accepts: DIAG_NORMAL with one |q_i| in [1e153, 1e155] (q²
+    overflows beyond 1.34e154) and the funnel with v in ±[700, 746] (exp(−v) overflows or is subnormal).  Where the
+    oracle raises the leapfrog ArgumentError the machine flags exactly that; everywhere else the
+    tree equals the oracle's bit for bit with status 0."""
+    import pyoracle as po
+    rng = np.random.default_rng(2)
+    seen = {1: [0, 0], 2: [0, 0]}
+    for family in (1, 2):
+        for trial in range(250):
+            D = int(rng.choice([2, 4, 10]))
+            q = rng.normal(size=D)
+            if family == 1:
+                params = np.concatenate([rng.normal(size=D), rng.uniform(0.5, 2, D)])
+                q[rng.integers(D)] = rng.choice([-1, 1]) * np.exp(rng.uniform(np.log(1e153), np.log(1e155)))
+            else:
+                params = None
+                q[0] = rng.uniform(-746, -700) if trial % 2 else rng.uniform(700, 746)
+                q[1:] *= np.exp(rng.uniform(-5, 5))
+            try:
+                po.evaluate_l(family, q, params, strict=True)
+            except po.OracleError:
+                continue
+            eps = float(np.exp(rng.uniform(-3, 1)))
+            h = hs.run(family, q, eps, 1, trial, params=params)
+            out = {}
+            if _raises_leapfrog_argcheck(po, lambda: out.update(po.sample_tree(family, q, eps, 1, trial, 0, params=params))):
+                assert h["status"] == LEAPFROG_NONFINITE, (family, trial)
+                seen[family][0] += 1
+            else:
+                assert h["status"] == 0, (family, trial)
+                _same_stats(out["stats"], h["tree_statistics"][0])
+                assert np.array_equal(out["q"], h["q"]) and np.array_equal(out["g"], h["g"]) and out["lq"] == h["lq"]
+                seen[family][1] += 1
+    assert all(a >= 20 and b >= 20 for a, b in seen.values()), seen
