@@ -181,26 +181,13 @@ __global__ void k_cov_pool(const double* covt, const double* means, double* minv
     __syncthreads();
   }
 }
-__global__ void k_broadcast_mat(double* dst, const double* src, size_t dd, size_t B) {
-  const size_t n = dd * B;
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-    dst[i] = src[i % dd];
-}
-
-// Mp[c][i][j] = M[c][i][j] for i, j < D, zero elsewhere ([B][rows][xs])
-__global__ void k_pad_metric(const double* M, double* Mp, size_t D, size_t rows, size_t xs, size_t B) {
+// Xp[c][n][j] = X[c][n][j] for n < N, j < D, zero elsewhere: B matrices [N][D] into [B][rows][xs]
+// (the rows of X, B = 1; every chain's M⁻¹, N = D)
+__global__ void k_pad_rows(const double* X, double* Xp, size_t N, size_t D, size_t rows, size_t xs, size_t B) {
   const size_t per = rows * xs, tot = per * B;
   for (size_t t = blockIdx.x * (size_t)blockDim.x + threadIdx.x; t < tot; t += (size_t)gridDim.x * blockDim.x) {
-    const size_t c = t / per, r = t % per, i = r / xs, j = r % xs;
-    Mp[t] = (i < D && j < D) ? M[c * D * D + i * D + j] : 0.0;
-  }
-}
-// Xp[n][j] = X[n][j] for n < N, j < D, zero elsewhere (rows x xs)
-__global__ void k_pad_rows(const double* X, double* Xp, size_t N, size_t D, size_t rows, size_t xs) {
-  const size_t tot = rows * xs;
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < tot; i += (size_t)gridDim.x * blockDim.x) {
-    const size_t n = i / xs, j = i % xs;
-    Xp[i] = (n < N && j < D) ? X[n * D + j] : 0.0;
+    const size_t c = t / per, r = t % per, n = r / xs, j = r % xs;
+    Xp[t] = (n < N && j < D) ? X[c * N * D + n * D + j] : 0.0;
   }
 }
 // Xt[j][n] = X[n][j], rows of Xt padded to ld >= N (pad = 0)
@@ -386,7 +373,21 @@ static std::string g_create_err;
 static bool needs_staging(const dhmc_handle* h) {
   return h->minv_dense || h->cfg.family == DHMC_FAMILY_LOGISTIC || h->cfg.family == DHMC_FAMILY_USER;
 }
-static int kernel_part(const dhmc_handle* h, KernelId k, int G);
+// The instantiation of kernel k for the handle's family, layout and metric kind.  Part 3: the deep persistent kernels;
+// part 1: the persistent kernels of packed chain groups (the light kernels run one chain per CTA); part 0: the rest.
+static const void* handle_kernel(dhmc_handle* h, KernelId k) {
+  const bool heavy = (k == K_NUTS || k == K_SEARCH);
+  const int part = heavy && h->deep ? 3 : heavy && h->G > 1 ? 1 : 0;
+  const void* fn = lookup_kernel(h->cfg.family, part, h->W, h->EPL, k, h->dense);
+  if (!fn) h->err = "kernel not built into this library for this layout (max_depth > 12 needs a user-model library built with its deep part: USER_PARTS=\"0 3\" / deep=True)";
+  return fn;
+}
+
+// whole blocks of 32 rows: the unit of the bulk copies into the tensor-core rounds (coop_core_tma, coop_matvec_tma)
+static size_t tma_rows(size_t n) { return (n + kTmaRows - 1) / kTmaRows * kTmaRows; }
+
+// grid of the dense-metric kernels (factor, window estimate): 4 CTAs per SM, no more than one per chain
+static int factor_grid(const dhmc_handle* h) { return (int)std::min<size_t>((size_t)h->sm_count * 4, (size_t)h->cfg.n_chains); }
 
 // rows of N doubles in the logistic scratch (residuals): one per CTA of the light kernels and, with one chain per CTA,
 // of the persistent kernels (packed groups keep theirs in shared memory)
@@ -411,8 +412,8 @@ static int plan(dhmc_handle* h) {
   h->smem_light = smem_layout(h->W, 0, slot_doubles, xs).total;      // light kernels: standard layout
   int& reg_ctas = h->reg_ctas[h->dense ? 1 : 0];
   if (reg_ctas == 0) {
-    const void* fn = lookup_kernel(h->cfg.family, kernel_part(h, K_NUTS, G), h->W, h->EPL, K_NUTS, h->dense);
-    if (!fn) { h->err = "kernel not built into this library for this layout (max_depth > 12 needs a user-model library built with its deep part: USER_PARTS=\"0 3\" / deep=True)"; return DHMC_EARG; }
+    const void* fn = handle_kernel(h, K_NUTS);
+    if (!fn) return DHMC_EARG;
     cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L0.total);
     if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&reg_ctas, fn, T * G, L0.total);
     if (e != cudaSuccess) { h->err = std::string("occupancy query: ") + cudaGetErrorString(e); return DHMC_ECUDA; }
@@ -437,12 +438,6 @@ static int plan(dhmc_handle* h) {
     CK(cudaMalloc(&h->lr, sizeof(double) * (size_t)h->lN * lr_rows(h)));
   }
   return DHMC_OK;
-}
-
-static int kernel_part(const dhmc_handle* h, KernelId k, int G) {
-  const bool heavy = (k == K_NUTS || k == K_SEARCH);
-  if (heavy && h->deep) return 3;
-  return G > 1 ? 1 : 0;
 }
 
 static int ensure_tmp(dhmc_handle* h, size_t doubles) {      // grow-only device scratch shared by the small entry points
@@ -477,10 +472,7 @@ static KArgs base_args(dhmc_handle* h) {
   return a;
 }
 
-// heavy = persistent kernels that use the slot pool (k_nuts, k_search)
-// timing: 0 = none, 1 = record ev0 before / ev1 after and read the time (synchronises),
-// 2 = record ev0 only (first of a series), 3 = record ev1 only (last; caller reads),
-// 4 = middle of a series.  reset_steps: zero the Σ steps counter first.
+// dhmc_last_kernel_ms: the time from ev0 to ev1 (synchronises)
 static int read_timer(dhmc_handle* h) {
   CK(cudaEventSynchronize(h->ev1));
   float ms = 0;
@@ -488,7 +480,9 @@ static int read_timer(dhmc_handle* h) {
   h->last_ms = ms;
   return DHMC_OK;
 }
-static int launch(dhmc_handle* h, KernelId k, KArgs a, int timing, bool reset_steps = true) {
+// heavy = persistent kernels that use the slot pool (k_nuts, k_search).  before / after (null: none) are recorded right
+// before and right after the kernel, so that they time it alone.  reset_steps: zero the Σ steps counter first.
+static int launch(dhmc_handle* h, KernelId k, KArgs a, cudaEvent_t before, cudaEvent_t after, bool reset_steps = true) {
   const bool heavy = (k == K_NUTS || k == K_SEARCH);
   if (!heavy) { a.n_sm = 0; }
   const size_t smem = heavy ? h->smem_bytes : smem_layout(h->W, 0, a.stride, (size_t)a.xs_doubles).total;
@@ -499,10 +493,10 @@ static int launch(dhmc_handle* h, KernelId k, KArgs a, int timing, bool reset_st
     CK(cudaMemsetAsync(h->counter, 0, sizeof(unsigned), h->stream));
     if (reset_steps) CK(cudaMemsetAsync(h->total_steps, 0, sizeof(unsigned long long), h->stream));
   }
-  if (timing == 1 || timing == 2) CK(cudaEventRecord(h->ev0, h->stream));
+  if (before) CK(cudaEventRecord(before, h->stream));
   {
-    const void* fn = lookup_kernel(h->cfg.family, kernel_part(h, k, G), h->W, h->EPL, k, h->dense);
-    if (!fn) { h->err = "kernel not built into this library for this layout (max_depth > 12 needs a user-model library built with its deep part: USER_PARTS=\"0 3\" / deep=True)"; return DHMC_EARG; }
+    const void* fn = handle_kernel(h, k);
+    if (!fn) return DHMC_EARG;
     cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) { h->err = std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(e); return DHMC_ECUDA; }
     void* params[] = {(void*)&a};
@@ -510,8 +504,7 @@ static int launch(dhmc_handle* h, KernelId k, KArgs a, int timing, bool reset_st
     if (e != cudaSuccess) { h->err = std::string("cudaLaunchKernel: ") + cudaGetErrorString(e); return DHMC_ECUDA; }
   }
   h->launches += 1;
-  if (timing == 1 || timing == 3) CK(cudaEventRecord(h->ev1, h->stream));
-  if (timing == 1) return read_timer(h);
+  if (after) CK(cudaEventRecord(after, h->stream));
   return DHMC_OK;
 }
 
@@ -712,62 +705,30 @@ int dhmc_user_family_name(char* name, size_t cap) {
   return DHMC_OK;
 }
 
-static void clear_batch(dhmc_handle* h) {
-  h->batch_k = h->batch_p = 0;
-  cudaFree(h->problems); h->problems = nullptr;
-}
-
-int dhmc_set_problem(dhmc_handle* h, const double* params, size_t n) {
-  if (!h) return DHMC_EARG;
-  CK(cudaSetDevice(h->cfg.device));
+// Checks one parameter block of the handle's family, blk[0 .. len); `who` names the entry point in the messages.
+static int check_block(dhmc_handle* h, const char* who, const double* blk, size_t len) {
   const size_t D = (size_t)h->cfg.dim;
-  if (h->cfg.family == DHMC_FAMILY_LOGISTIC) {
-    // params = [N, X row-major (N×D), y (N)]
-    if (!params || n < 1) { h->err = "dhmc_set_problem: logistic regression needs [N, X, y]"; return DHMC_EARG; }
-    const size_t N = (size_t)params[0];
-    if (N < 1 || n != 1 + N * D + N) { h->err = "dhmc_set_problem: expected 1 + N*D + N values"; return DHMC_EARG; }
-    for (size_t i = 0; i < N; ++i) {       // the model is a Bernoulli likelihood: responses (or their means) in [0, 1]
-      const double yv = params[1 + N * D + i];
-      if (!(yv >= 0.0 && yv <= 1.0)) { h->err = "dhmc_set_problem: logistic regression needs 0 <= y <= 1"; return DHMC_EARG; }
+  auto fail = [&](const char* m) { h->err = std::string(who) + ": " + m; return DHMC_EARG; };
+  switch (h->cfg.family) {
+    case DHMC_FAMILY_USER:                 // any number of doubles, interpreted by the user's formulas
+      return len && !blk ? fail("null parameter block") : DHMC_OK;
+    case DHMC_FAMILY_DIAG_NORMAL:
+      return len != 2 * D || !blk ? fail("DIAG_NORMAL blocks are [mu(D), prec(D)]") : DHMC_OK;
+    case DHMC_FAMILY_LOGISTIC: {
+      if (!blk || len < 1) return fail("logistic blocks are [N, X (N*D), y (N)]");
+      const double v = blk[0];
+      if (!(v >= 1.0 && v < 2147483648.0 && v == std::floor(v))) return fail("a logistic block starts with its N, an integer with 1 <= N < 2^31");
+      const size_t N = (size_t)v;
+      if (len != 1 + N * D + N) return fail("logistic blocks are [N, X (N*D), y (N)]: a block's length disagrees with its N");
+      for (size_t i = 0; i < N; ++i) {     // the model is a Bernoulli likelihood: responses (or their means) in [0, 1]
+        const double yv = blk[1 + N * D + i];
+        if (!(yv >= 0.0 && yv <= 1.0)) return fail("logistic regression needs 0 <= y <= 1");
+      }
+      return DHMC_OK;
     }
-    clear_batch(h);
-    cudaFree(h->lX); cudaFree(h->lXt); cudaFree(h->ly); cudaFree(h->lr); cudaFree(h->lXp);
-    h->lX = h->lXt = h->ly = h->lr = h->lXp = nullptr;
-    const size_t ld = (N + 1) & ~(size_t)1;                 // even leading dimension: 16-byte aligned row segments
-    CK(cudaMalloc(&h->lX, sizeof(double) * N * D));
-    CK(cudaMalloc(&h->lXt, sizeof(double) * ld * D));
-    CK(cudaMalloc(&h->ly, sizeof(double) * N));
-    CK(cudaMalloc(&h->lr, sizeof(double) * N * lr_rows(h)));
-    CK(cudaMemcpyAsync(h->lX, params + 1, sizeof(double) * N * D, cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemcpyAsync(h->ly, params + 1 + N * D, sizeof(double) * N, cudaMemcpyHostToDevice, h->stream));
-    k_transpose<<<1024, 256, 0, h->stream>>>(h->lX, h->lXt, N, D, ld);
-    h->launches += 1;
-    if (h->G > 1) {   // row blocks [32][XS] with zero padding (rows >= N, columns >= D): one bulk copy per block
-      const size_t xs = (size_t)tma_xs((int)D), rows = (N + kTmaRows - 1) / kTmaRows * kTmaRows;
-      CK(cudaMalloc(&h->lXp, sizeof(double) * rows * xs));
-      k_pad_rows<<<1024, 256, 0, h->stream>>>(h->lX, h->lXp, N, D, rows, xs);
-      h->launches += 1;
-    }
-    h->lN = (int)N; h->lLd = (int)ld;
-    CK(cudaStreamSynchronize(h->stream));
-    return DHMC_OK;
+    default:                               // STD_NORMAL, FUNNEL
+      return len ? fail("this family has no parameters (n == 0)") : DHMC_OK;
   }
-  if (h->cfg.family == DHMC_FAMILY_USER) {      // any number of doubles, interpreted by the user's formulas
-    if (n && !params) { h->err = "dhmc_set_problem: null parameter block"; return DHMC_EARG; }
-    clear_batch(h);
-    CK(cudaStreamSynchronize(h->stream));
-    cudaFree(h->mparams); h->mparams = nullptr;
-    CK(cudaMalloc(&h->mparams, sizeof(double) * std::max<size_t>(n, 1)));
-    if (n) CK(cudaMemcpyAsync(h->mparams, params, sizeof(double) * n, cudaMemcpyHostToDevice, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    return DHMC_OK;
-  }
-  const size_t want = h->cfg.family == DHMC_FAMILY_DIAG_NORMAL ? 2 * D : 0;
-  if (n != want || (want && !params)) { h->err = "dhmc_set_problem: wrong parameter count for this family"; return DHMC_EARG; }
-  clear_batch(h);                                // (mparams holds at least 2·D doubles, also after a batch)
-  if (want) CK(cudaMemcpyAsync(h->mparams, params, sizeof(double) * want, cudaMemcpyHostToDevice, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  return DHMC_OK;
 }
 
 // The checks every problem batch shares (dhmc_set_problems, dhmc_set_problems_ragged); `who` names the entry point in the
@@ -788,10 +749,11 @@ static int check_batch(dhmc_handle* h, const char* who, bool have_blocks, int64_
   return DHMC_OK;
 }
 
-// Installs P validated blocks (problem p: params[offs[p] .. offs[p+1])), each sampled by K chains.  Every problem gets arrays of
-// its own size, back to back, and a descriptor that says where they start.  The new arrays are complete before they replace
-// the current ones: on any error the previous problem (batch or not) stays in effect.
-static int install_batch(dhmc_handle* h, const double* params, const std::vector<size_t>& offs, int64_t P, int64_t K) {
+// Installs P validated blocks (problem p: params[offs[p] .. offs[p+1])), each sampled by K chains; K = 0: one problem
+// (P = 1) for every chain, and no descriptor table.  Every problem gets arrays of its own size, back to back, and a
+// descriptor that says where they start.  The new arrays are complete before they replace the current ones: on any error
+// the previous problem (batch or not) stays in effect.
+static int install_problems(dhmc_handle* h, const double* params, const std::vector<size_t>& offs, int64_t P, int64_t K) {
   const int fam = h->cfg.family;
   const size_t D = (size_t)h->cfg.dim, Pz = (size_t)P;
   const size_t xs = fam == DHMC_FAMILY_LOGISTIC ? (size_t)tma_xs((int)D) : 0;
@@ -803,9 +765,8 @@ static int install_batch(dhmc_handle* h, const double* params, const std::vector
     if (fam != DHMC_FAMILY_LOGISTIC) { d.mparams = offs[p]; continue; }
     const size_t N = (size_t)params[offs[p]];
     const size_t ld = (N + 1) & ~(size_t)1;                     // even leading dimension: 16-byte aligned row segments
-    const size_t rows = (N + kTmaRows - 1) / kTmaRows * kTmaRows; // whole row blocks of [32][xs] for the bulk copies
     d.X = tX; d.Xt = tXt; d.y = ty; d.Xp = h->G > 1 ? tXp : 0; d.N = (int)N; d.ld = (int)ld;
-    tX += N * D; tXt += ld * D; ty += N; tXp += rows * xs;
+    tX += N * D; tXt += ld * D; ty += N; tXp += tma_rows(N) * xs;
     maxN = std::max(maxN, N);
     if (d.Xt % 2 != 0 || (h->G > 1 && d.Xp % (kTmaRows * xs) != 0)) {
       h->err = "problem batch: misaligned problem base in X^T or padded X (internal error)"; return DHMC_ECUDA;
@@ -818,8 +779,10 @@ static int install_batch(dhmc_handle* h, const double* params, const std::vector
   auto drop = [&] { cudaFree(mp); cudaFree(X); cudaFree(Xt); cudaFree(y); cudaFree(Xp); cudaFree(lr); cudaFree(dd); };
 #define CKB(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { h->err = std::string(#call) + ": " + cudaGetErrorString(e_); \
     cudaStreamSynchronize(h->stream); drop(); return e_ == cudaErrorMemoryAllocation ? DHMC_ENOMEM : DHMC_ECUDA; } } while (0)
-  CKB(cudaMalloc(&dd, sizeof(ProblemDesc) * Pz));
-  CKB(cudaMemcpyAsync(dd, desc.data(), sizeof(ProblemDesc) * Pz, cudaMemcpyHostToDevice, h->stream));
+  if (K) {
+    CKB(cudaMalloc(&dd, sizeof(ProblemDesc) * Pz));
+    CKB(cudaMemcpyAsync(dd, desc.data(), sizeof(ProblemDesc) * Pz, cudaMemcpyHostToDevice, h->stream));
+  }
   if (fam == DHMC_FAMILY_LOGISTIC) {
     // per problem: X [N][D], Xᵀ [D][ld], y [N] and, for packed groups, the zero-padded row blocks [rows][xs]; one residual
     // scratch of rows of the largest N
@@ -835,12 +798,13 @@ static int install_batch(dhmc_handle* h, const double* params, const std::vector
       CKB(cudaMemcpyAsync(X + d.X, blk + 1, sizeof(double) * N * D, cudaMemcpyHostToDevice, h->stream));
       CKB(cudaMemcpyAsync(y + d.y, blk + 1 + N * D, sizeof(double) * N, cudaMemcpyHostToDevice, h->stream));
       k_transpose<<<1024, 256, 0, h->stream>>>(X + d.X, Xt + d.Xt, N, D, (size_t)d.ld);
-      if (Xp) k_pad_rows<<<1024, 256, 0, h->stream>>>(X + d.X, Xp + d.Xp, N, D, (N + kTmaRows - 1) / kTmaRows * kTmaRows, xs);
+      if (Xp) k_pad_rows<<<1024, 256, 0, h->stream>>>(X + d.X, Xp + d.Xp, N, D, tma_rows(N), xs, 1);
       h->launches += Xp ? 2 : 1;
     }
-  } else {
-    CKB(cudaMalloc(&mp, sizeof(double) * offs[Pz]));
-    CKB(cudaMemcpyAsync(mp, params, sizeof(double) * offs[Pz], cudaMemcpyHostToDevice, h->stream));
+  } else if (fam == DHMC_FAMILY_DIAG_NORMAL || fam == DHMC_FAMILY_USER) {   // (STD_NORMAL and FUNNEL have no parameters)
+    // mparams is never null, also for a USER model without parameters
+    CKB(cudaMalloc(&mp, sizeof(double) * std::max<size_t>(offs[Pz], 1)));
+    if (offs[Pz]) CKB(cudaMemcpyAsync(mp, params, sizeof(double) * offs[Pz], cudaMemcpyHostToDevice, h->stream));
   }
   CKB(cudaGetLastError());
   CKB(cudaStreamSynchronize(h->stream));
@@ -849,74 +813,56 @@ static int install_batch(dhmc_handle* h, const double* params, const std::vector
     cudaFree(h->lX); cudaFree(h->lXt); cudaFree(h->ly); cudaFree(h->lr); cudaFree(h->lXp);
     h->lX = X; h->lXt = Xt; h->ly = y; h->lr = lr; h->lXp = Xp;
     h->lN = (int)maxN; h->lLd = desc[0].ld;    // a chain's own N and ld come from its descriptor
-  } else {
+  } else if (mp) {
     cudaFree(h->mparams);
     h->mparams = mp;
   }
   cudaFree(h->problems);
   h->problems = dd;
-  h->batch_k = K; h->batch_p = P;
+  h->batch_k = K; h->batch_p = K ? P : 0;
   return DHMC_OK;
+}
+
+int dhmc_set_problem(dhmc_handle* h, const double* params, size_t n) {
+  if (!h) return DHMC_EARG;
+  if (int rc = check_block(h, "dhmc_set_problem", params, n)) return rc;
+  return install_problems(h, params, {0, n}, 1, 0);
 }
 
 // P problems of the handle's family and dimension, each with its own parameter block of n doubles; global chain g samples
 // problem g / chains_per_problem.  Everything is validated before anything is allocated.
 int dhmc_set_problems(dhmc_handle* h, const double* params, size_t n, int64_t P, int64_t K) {
   if (!h) return DHMC_EARG;
-  const int fam = h->cfg.family;
-  const size_t D = (size_t)h->cfg.dim;
   if (int rc = check_batch(h, "dhmc_set_problems", params && n >= 1, P, K)) return rc;
-  size_t N = 0;
-  if (fam == DHMC_FAMILY_DIAG_NORMAL && n != 2 * D) { h->err = "dhmc_set_problems: DIAG_NORMAL blocks are [mu(D), prec(D)]"; return DHMC_EARG; }
-  if (fam == DHMC_FAMILY_LOGISTIC) {
-    N = params[0] >= 1 ? (size_t)params[0] : 0;
-    if (N < 1 || n != 1 + N * D + N) { h->err = "dhmc_set_problems: logistic blocks are [N, X (N*D), y (N)]"; return DHMC_EARG; }
-    for (int64_t p = 0; p < P; ++p) {
-      const double* blk = params + (size_t)p * n;
-      if (blk[0] != params[0]) { h->err = "dhmc_set_problems: every logistic problem of a batch needs the same N"; return DHMC_EARG; }
-      for (size_t i = 0; i < N; ++i) {
-        const double yv = blk[1 + N * D + i];
-        if (!(yv >= 0.0 && yv <= 1.0)) { h->err = "dhmc_set_problems: logistic regression needs 0 <= y <= 1"; return DHMC_EARG; }
-      }
-    }
-  }
+  if (h->cfg.family == DHMC_FAMILY_LOGISTIC)
+    for (int64_t p = 1; p < P; ++p)
+      if (params[(size_t)p * n] != params[0]) { h->err = "dhmc_set_problems: every logistic problem of a batch needs the same N"; return DHMC_EARG; }
   std::vector<size_t> offs((size_t)P + 1);
   for (size_t p = 0; p <= (size_t)P; ++p) offs[p] = p * n;
-  return install_batch(h, params, offs, P, K);
+  for (int64_t p = 0; p < P; ++p)
+    if (int rc = check_block(h, "dhmc_set_problems", params + offs[p], n)) return rc;
+  return install_problems(h, params, offs, P, K);
 }
 
 // The same with blocks of different lengths: problem p's block is params[block_offsets[p] .. block_offsets[p+1]).
 int dhmc_set_problems_ragged(dhmc_handle* h, const double* params, const size_t* offs, int64_t P, int64_t K) {
   if (!h) return DHMC_EARG;
-  const int fam = h->cfg.family;
-  const size_t D = (size_t)h->cfg.dim;
-  if (int rc = check_batch(h, "dhmc_set_problems_ragged", params && offs, P, K)) return rc;
-  auto fail = [&](const char* m) { h->err = std::string("dhmc_set_problems_ragged: ") + m; return DHMC_EARG; };
+  const char* who = "dhmc_set_problems_ragged";
+  if (int rc = check_batch(h, who, params && offs, P, K)) return rc;
+  auto fail = [&](const char* m) { h->err = std::string(who) + ": " + m; return DHMC_EARG; };
   if (offs[0] != 0) return fail("block_offsets[0] must be 0");
   for (int64_t p = 0; p < P; ++p)
     if (offs[p + 1] <= offs[p]) return fail("block_offsets must strictly increase (every block holds at least one value)");
-  for (int64_t p = 0; p < P; ++p) {
-    const double* blk = params + offs[p];
-    const size_t len = offs[p + 1] - offs[p];
-    if (fam == DHMC_FAMILY_DIAG_NORMAL && len != 2 * D) return fail("DIAG_NORMAL blocks are [mu(D), prec(D)]");
-    if (fam != DHMC_FAMILY_LOGISTIC) continue;
-    const double v = blk[0];
-    if (!(v >= 1.0 && v < 2147483648.0 && v == std::floor(v))) return fail("a logistic block starts with its N, an integer with 1 <= N < 2^31");
-    const size_t N = (size_t)v;
-    if (len != 1 + N * D + N) return fail("logistic blocks are [N, X (N*D), y (N)]: a block's length disagrees with its N");
-    for (size_t i = 0; i < N; ++i) {
-      const double yv = blk[1 + N * D + i];
-      if (!(yv >= 0.0 && yv <= 1.0)) return fail("logistic regression needs 0 <= y <= 1");
-    }
-  }
-  return install_batch(h, params, std::vector<size_t>(offs, offs + P + 1), P, K);
+  for (int64_t p = 0; p < P; ++p)
+    if (int rc = check_block(h, who, params + offs[p], offs[p + 1] - offs[p])) return rc;
+  return install_problems(h, params, std::vector<size_t>(offs, offs + P + 1), P, K);
 }
 
 static int eval_position(dhmc_handle* h, bool randomize) {
   CK(cudaMemsetAsync(h->status, 0, sizeof(int) * (size_t)h->cfg.n_chains, h->stream));
   KArgs a = base_args(h);
   a.strict = 1; a.randomize = randomize ? 1 : 0;
-  int rc = launch(h, K_EVAL, a, 0);
+  int rc = launch(h, K_EVAL, a, nullptr, nullptr);
   if (rc != DHMC_OK) return rc;
   h->has_position = true;
   return sync_and_check_status(h, DHMC_CHAIN_BAD_INITIAL, "initialize_warmup_state: invalid log density or gradient at the initial position");
@@ -941,32 +887,34 @@ static int ensure_dense(dhmc_handle* h) {
   CK(cudaMalloc(&h->minv_dense, sizeof(double) * B * dd));
   CK(cudaMalloc(&h->wt, sizeof(double) * B * dd));
   CK(cudaMalloc(&h->covt, sizeof(double) * B * dd));
-  const int fgrid = (int)std::min<size_t>((size_t)h->sm_count * 4, B);
-  CK(cudaMalloc(&h->dense_tmp, sizeof(double) * 3 * dd * (size_t)fgrid));
+  CK(cudaMalloc(&h->dense_tmp, sizeof(double) * 3 * dd * (size_t)factor_grid(h)));
   CK(cudaMemsetAsync(h->wt, 0, sizeof(double) * B * dd, h->stream));
-  if (h->G > 1) {   // [B][⌈D/32⌉·32][XS]: one bulk copy per 32-row block (coop_matvec_tma)
-    const size_t rows = ((size_t)h->cfg.dim + kTmaRows - 1) / kTmaRows * kTmaRows;
-    CK(cudaMalloc(&h->minv_pad, sizeof(double) * B * rows * (size_t)tma_xs((int)h->cfg.dim)));
-  }
-  return plan(h);   // the shared-memory layout now carries the mat-vec staging vector
+  if (h->G > 1)     // [B][⌈D/32⌉·32][XS]: one bulk copy per 32-row block (coop_matvec_tma)
+    CK(cudaMalloc(&h->minv_pad, sizeof(double) * B * tma_rows((size_t)h->cfg.dim) * (size_t)tma_xs((int)h->cfg.dim)));
+  // re-planned whatever the metric kind: with the dense arrays allocated, the shared-memory layout carries the staging
+  // vector (needs_staging) also for the diagonal kernels
+  return plan(h);
+}
+// The metric kind of the handle's kernels: the persistent kernels are re-planned when the slot width (dense) changes.
+static int set_metric_kind(dhmc_handle* h, bool dense, bool pooled) {
+  h->pooled = pooled;
+  if (h->dense == dense) return DHMC_OK;
+  h->dense = dense;
+  return plan(h);
 }
 // κ = GaussianKineticEnergy(Symmetric M⁻¹): W = cholesky(inv(M⁻¹)).L on device, then switch
-// the handle to the dense kernels.
-static int factor_and_switch(dhmc_handle* h) {
-  const size_t B = (size_t)h->cfg.n_chains;
-  const int fgrid = (int)std::min<size_t>((size_t)h->sm_count * 4, B);
+// the handle to the dense kernels (pooled: M⁻¹ is shared by every group of 8 chains).
+static int factor_and_switch(dhmc_handle* h, bool pooled) {
+  const size_t B = (size_t)h->cfg.n_chains, D = (size_t)h->cfg.dim;
   CK(cudaMemsetAsync(h->status, 0, sizeof(int) * B, h->stream));
-  k_dense_factor<<<fgrid, 128, 0, h->stream>>>(h->minv_dense, h->wt, h->dense_tmp, h->status, (int)h->cfg.dim, (int)B);
+  k_dense_factor<<<factor_grid(h), 128, 0, h->stream>>>(h->minv_dense, h->wt, h->dense_tmp, h->status, (int)D, (int)B);
   h->launches += 1;
   if (h->minv_pad) {
-    const size_t rows = ((size_t)h->cfg.dim + kTmaRows - 1) / kTmaRows * kTmaRows;
-    k_pad_metric<<<2048, 256, 0, h->stream>>>(h->minv_dense, h->minv_pad, (size_t)h->cfg.dim, rows, (size_t)tma_xs((int)h->cfg.dim), B);
+    k_pad_rows<<<2048, 256, 0, h->stream>>>(h->minv_dense, h->minv_pad, D, D, tma_rows(D), (size_t)tma_xs((int)D), B);
     h->launches += 1;
   }
   CK(cudaGetLastError());
-  const bool was = h->dense;
-  h->dense = true;
-  if (!was) { int rc = plan(h); if (rc != DHMC_OK) return rc; }
+  if (int rc = set_metric_kind(h, true, pooled)) return rc;
   return sync_and_check_status(h, DHMC_CHAIN_NOT_POSDEF, "GaussianKineticEnergy: M⁻¹ is not positive definite (PosDefException)");
 }
 
@@ -975,19 +923,18 @@ int dhmc_set_metric_dense(dhmc_handle* h, const double* minv, int broadcast) {
   CK(cudaSetDevice(h->cfg.device));
   int rc = ensure_dense(h);
   if (rc != DHMC_OK) return rc;
-  h->pooled = false;
   const size_t B = (size_t)h->cfg.n_chains, dd = (size_t)h->cfg.dim * h->cfg.dim;
   if (broadcast) {
     int rct = ensure_tmp(h, dd);
     if (rct != DHMC_OK) return rct;
     CK(cudaMemcpyAsync(h->tmp_bd, minv, sizeof(double) * dd, cudaMemcpyHostToDevice, h->stream));
-    k_broadcast_mat<<<1024, 256, 0, h->stream>>>(h->minv_dense, h->tmp_bd, dd, B);
+    k_broadcast<<<1024, 256, 0, h->stream>>>(h->minv_dense, h->tmp_bd, dd, B);
     h->launches += 1;
     CK(cudaStreamSynchronize(h->stream));
   } else {
     CK(cudaMemcpyAsync(h->minv_dense, minv, sizeof(double) * B * dd, cudaMemcpyHostToDevice, h->stream));
   }
-  return factor_and_switch(h);
+  return factor_and_switch(h, false);
 }
 int dhmc_get_metric_dense(dhmc_handle* h, double* minv) {
   if (!h || !minv) return DHMC_EARG;
@@ -1015,9 +962,7 @@ int dhmc_set_metric(dhmc_handle* h, const double* minv, int broadcast) {
   }
   h->launches += 1;
   CK(cudaStreamSynchronize(h->stream));
-  h->pooled = false;
-  if (h->dense) { h->dense = false; int rc = plan(h); if (rc != DHMC_OK) return rc; }
-  return DHMC_OK;
+  return set_metric_kind(h, false, false);
 }
 
 int dhmc_set_stepsize(dhmc_handle* h, const double* eps, int broadcast) {
@@ -1075,7 +1020,8 @@ int dhmc_leapfrog(dhmc_handle* h, int32_t n_steps, int32_t sign) {
   CK(cudaMemsetAsync(h->status, 0, sizeof(int) * (size_t)h->cfg.n_chains, h->stream));   // status words describe the current call
   KArgs a = base_args(h);
   a.lf_steps = n_steps; a.lf_sign = sign;
-  int rc = launch(h, K_LEAPFROG, a, 1);
+  int rc = launch(h, K_LEAPFROG, a, h->ev0, h->ev1);
+  if (rc == DHMC_OK) rc = read_timer(h);
   if (rc != DHMC_OK) return rc;
   return sync_and_check_status(h, DHMC_CHAIN_NONFINITE_Q | DHMC_CHAIN_LEAPFROG_NONFINITE,
                                "leapfrog: position vector has non-finite elements");
@@ -1089,7 +1035,7 @@ int dhmc_phase_logdensity(dhmc_handle* h, double* out) {
   if (rc != DHMC_OK) return rc;
   KArgs a = base_args(h);
   a.out_phase = h->tmp_b;
-  rc = launch(h, K_PHASE, a, 0);
+  rc = launch(h, K_PHASE, a, nullptr, nullptr);
   if (rc != DHMC_OK) return rc;
   CK(cudaMemcpyAsync(out, h->tmp_b, sizeof(double) * B, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
@@ -1108,7 +1054,8 @@ int dhmc_find_initial_stepsize(dhmc_handle* h, double initial_eps, double log_th
   CK(cudaMemsetAsync(h->status, 0, sizeof(int) * (size_t)h->cfg.n_chains, h->stream));   // status words describe the current call
   KArgs a = base_args(h);
   a.s_init = initial_eps; a.s_thresh = log_threshold; a.s_maxiter = maxiter;
-  int rc = launch(h, K_SEARCH, a, 1);
+  int rc = launch(h, K_SEARCH, a, h->ev0, h->ev1);
+  if (rc == DHMC_OK) rc = read_timer(h);
   if (rc != DHMC_OK) return rc;
   // the reference aborts when the search fails (stepsize.jl:58,78): ϵ counts as set only if every chain found one
   rc = sync_and_check_status(h, DHMC_CHAIN_SEARCH_FAILED | DHMC_CHAIN_NONFINITE_Q,
@@ -1150,24 +1097,22 @@ static int run_nuts(dhmc_handle* h, int N, const AdaptConfig& cfg, double lambda
   CK(cudaSetDevice(h->cfg.device));
   if (thin < 1 || N % thin != 0) { h->err = "thin >= 1 and N a multiple of thin"; return DHMC_EARG; }
   const size_t B = (size_t)h->cfg.n_chains, D = (size_t)h->cfg.dim, n = (size_t)(N / thin);   // n: kept draws per chain
-  double *d_post = nullptr, *d_eps = nullptr, *d_ld = nullptr, *d_p = nullptr;
-  dhmc_tree_stats* d_stats = nullptr;
+  double* d_p = nullptr;
   unsigned* d_dir = nullptr;
   int rc = DHMC_OK;
-  auto cleanup = [&] {};              // (the override buffers are the handle's grow-only scratch)
-#define CKR(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { h->err = std::string(#call) + ": " + cudaGetErrorString(e_); cleanup(); return e_ == cudaErrorMemoryAllocation ? DHMC_ENOMEM : DHMC_ECUDA; } } while (0)
-#define CKS(call) do { int r_ = (call); if (r_ != DHMC_OK) { cleanup(); return r_; } } while (0)
   // Host outputs.  Page-locked (pinned) buffers are written by the kernel itself through their device alias — no staging
   // copy in HBM, no second hop, the PCIe writes overlap the sampling at cache-line granularity and N is not bounded by
-  // device memory.  Pageable buffers are staged in HBM and copied chunk by chunk; if the draws would not fit, the buffer
-  // is page-locked on the fly (cudaHostRegister) and written directly.
-  bool direct[4] = {false, false, false, false};
-  if (outputs_on_device) {
-    d_post = posterior; d_stats = stats; d_eps = eps_used; d_ld = logdens;
-  } else {
-    void* dv = nullptr;
-    if (posterior) {
-      const size_t bytes = sizeof(double) * B * n * D;
+  // device memory.  Pageable buffers are staged in HBM (out[i] in stage[i]) and copied chunk by chunk; if the draws would
+  // not fit, the buffer is page-locked on the fly (cudaHostRegister) and written directly.
+  struct Output { void* host; size_t row; void* dev; bool direct; };       // row: bytes per kept draw of a chain
+  Output out[4] = {{posterior, sizeof(double) * D, nullptr, false}, {stats, sizeof(dhmc_tree_stats), nullptr, false},
+                   {eps_used, sizeof(double), nullptr, false}, {logdens, sizeof(double), nullptr, false}};
+  for (int i = 0; i < 4; ++i) {
+    Output& o = out[i];
+    if (!o.host) continue;
+    if (outputs_on_device) { o.dev = o.host; continue; }
+    const size_t bytes = o.row * B * n;
+    if (i == 0) {
       // Draws: staging + DMA copies overlapped chunk by chunk is the faster route when the draws fit in HBM (C2: 21.9 ms per
       // step against 24.1 ms with direct writes — kernel stores reach ~47 GB/s over PCIe, the copy engines 57 GB/s); the
       // kernel writes the host buffer directly when they do not fit (DHMC_DIRECT=1 forces it).
@@ -1176,58 +1121,52 @@ static int run_nuts(dhmc_handle* h, int N, const AdaptConfig& cfg, double lambda
       const bool fits = bytes <= h->stage_bytes[0] || bytes + ((size_t)1 << 30) <= fr;
       const char* evd = std::getenv("DHMC_DIRECT");
       const bool force_direct = evd && std::atoi(evd) == 1;
-      bool ok = false;
       if (!fits || force_direct) {
-        ok = host_mapped(posterior, &dv);
-        if (!ok && !fits) {                                                         // pageable and too large: page-lock the caller's buffer
-          if (cudaHostRegister(posterior, bytes, cudaHostRegisterMapped) == cudaSuccess) {
-            h->registered.push_back(posterior);
-            ok = host_mapped(posterior, &dv);
+        o.direct = host_mapped(o.host, &o.dev);
+        if (!o.direct && !fits) {                                                   // pageable and too large: page-lock the caller's buffer
+          if (cudaHostRegister(o.host, bytes, cudaHostRegisterMapped) == cudaSuccess) {
+            h->registered.push_back(o.host);
+            o.direct = host_mapped(o.host, &o.dev);
           } else {
             cudaGetLastError();
           }
         }
       }
-      if (ok) { d_post = (double*)dv; direct[0] = true; }
-      else { CKS(ensure_stage(h, 0, bytes)); d_post = (double*)h->stage[0]; }
+    } else {
+      o.direct = host_mapped(o.host, &o.dev);
     }
-    if (stats) {
-      if (host_mapped(stats, &dv)) { d_stats = (dhmc_tree_stats*)dv; direct[1] = true; }
-      else { CKS(ensure_stage(h, 1, sizeof(dhmc_tree_stats) * B * n)); d_stats = (dhmc_tree_stats*)h->stage[1]; }
-    }
-    if (eps_used) {
-      if (host_mapped(eps_used, &dv)) { d_eps = (double*)dv; direct[2] = true; }
-      else { CKS(ensure_stage(h, 2, sizeof(double) * B * n)); d_eps = (double*)h->stage[2]; }
-    }
-    if (logdens) {
-      if (host_mapped(logdens, &dv)) { d_ld = (double*)dv; direct[3] = true; }
-      else { CKS(ensure_stage(h, 3, sizeof(double) * B * n)); d_ld = (double*)h->stage[3]; }
+    if (!o.direct) {
+      if ((rc = ensure_stage(h, i, bytes)) != DHMC_OK) return rc;
+      o.dev = h->stage[i];
     }
   }
-  if (p_over_host || dir_over_host) CKS(ensure_tmp(h, p_over_host ? B * D : 0));
+  if (p_over_host || dir_over_host) {
+    if ((rc = ensure_tmp(h, p_over_host ? B * D : 0)) != DHMC_OK) return rc;
+  }
   if (p_over_host) {
     d_p = h->tmp_bd;
-    CKR(cudaMemcpyAsync(d_p, p_over_host, sizeof(double) * B * D, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(d_p, p_over_host, sizeof(double) * B * D, cudaMemcpyHostToDevice, h->stream));
   }
   if (dir_over_host) {
     d_dir = h->tmp_dir;
-    CKR(cudaMemcpyAsync(d_dir, dir_over_host, sizeof(unsigned) * B, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(d_dir, dir_over_host, sizeof(unsigned) * B, cudaMemcpyHostToDevice, h->stream));
   }
   tr_pt[0] = tr_ms();
   KArgs a = base_args(h);
   a.N = N; a.thin = thin; a.N_keep = (int)n; a.cfg = cfg; a.p_override = d_p; a.dir_override = d_dir;
-  a.out_q = d_post; a.out_stats = d_stats; a.out_eps = d_eps; a.out_lq = d_ld;
+  a.out_q = (double*)out[0].dev; a.out_stats = (dhmc_tree_stats*)out[1].dev; a.out_eps = (double*)out[2].dev;
+  a.out_lq = (double*)out[3].dev;
   if (cfg.metric == DHMC_METRIC_SYMMETRIC) a.covt = h->covt;
   if (pool_metric) a.mean_out = h->mean_pool;
   const size_t out_bytes = posterior ? sizeof(double) * B * n * D : 0;
   // chunks must stay many waves long, or the ragged tail of every chunk idles the SMs
   // chunks overlap the staged downloads (and the upload of q_host) with the sampling of the next chunk; with direct
   // host writes only an upload is left to overlap
-  const bool staged_big = posterior && !direct[0] && out_bytes >= ((size_t)32 << 20);
+  const bool staged_big = posterior && !out[0].direct && out_bytes >= ((size_t)32 << 20);
   int nchunks = (!outputs_on_device && B >= 4096 && (staged_big || q_host)) ? 16 : 1;
   while (nchunks > 1 && B / (size_t)nchunks < (size_t)8 * (size_t)h->grid * (size_t)h->G) nchunks /= 2;   // >= 8 waves of chain slots per chunk
   if (const char* ev = std::getenv("DHMC_E2E_CHUNKS")) { const int v = std::atoi(ev); if (v >= 1 && v <= 16 && !outputs_on_device) nchunks = v; }
-  CKR(cudaMemsetAsync(h->status, 0, sizeof(int) * B, h->stream));   // status words describe the current call
+  CK(cudaMemsetAsync(h->status, 0, sizeof(int) * B, h->stream));   // status words describe the current call
   for (int ci = 0; ci < nchunks; ++ci) {
     // (a pooled metric, and a batch on packed groups, keep their groups of 8 chains inside one chunk)
     const size_t unit = (h->pooled || (h->G > 1 && h->batch_k)) ? 8 : 1;
@@ -1238,39 +1177,39 @@ static int run_nuts(dhmc_handle* h, int N, const AdaptConfig& cfg, double lambda
       // positions of this chunk: H2D on its own stream, then evaluate_ℓ(strict) on the compute
       // stream — overlaps with the previous chunk's sampling and D2H
       if (ci == 0) {   // uploads start after everything already queued on the compute stream
-        CKR(cudaEventRecord(h->h2d_ev[15], h->stream));
-        CKR(cudaStreamWaitEvent(h->h2d_stream, h->h2d_ev[15], 0));
+        CK(cudaEventRecord(h->h2d_ev[15], h->stream));
+        CK(cudaStreamWaitEvent(h->h2d_stream, h->h2d_ev[15], 0));
       }
-      CKR(cudaMemcpyAsync(h->q + c0 * D, q_host + c0 * D, sizeof(double) * nc * D, cudaMemcpyHostToDevice, h->h2d_stream));
-      CKR(cudaEventRecord(h->h2d_ev[ci], h->h2d_stream));
-      CKR(cudaStreamWaitEvent(h->stream, h->h2d_ev[ci], 0));
+      CK(cudaMemcpyAsync(h->q + c0 * D, q_host + c0 * D, sizeof(double) * nc * D, cudaMemcpyHostToDevice, h->h2d_stream));
+      CK(cudaEventRecord(h->h2d_ev[ci], h->h2d_stream));
+      CK(cudaStreamWaitEvent(h->stream, h->h2d_ev[ci], 0));
       KArgs ea = a;
       ea.strict = 1; ea.randomize = 0;
-      rc = launch(h, K_EVAL, ea, 0);
-      if (rc != DHMC_OK) { cleanup(); return rc; }
+      rc = launch(h, K_EVAL, ea, nullptr, nullptr);
+      if (rc != DHMC_OK) return rc;
     }
-    const int timing = nchunks == 1 ? 1 : (ci == 0 ? 2 : (ci == nchunks - 1 ? 3 : 4));
-    rc = launch(h, K_NUTS, a, timing == 1 ? 2 : timing, ci == 0);
-    if (rc != DHMC_OK) { cleanup(); return rc; }
-    if (nchunks == 1) CKR(cudaEventRecord(h->ev1, h->stream));
+    // the kernel time of the call: from the first chunk's k_nuts to the end of the last one's
+    rc = launch(h, K_NUTS, a, ci == 0 ? h->ev0 : nullptr, ci == nchunks - 1 ? h->ev1 : nullptr, ci == 0);
+    if (rc != DHMC_OK) return rc;
     if (!outputs_on_device) {
-      CKR(cudaEventRecord(h->chunk_ev[ci], h->stream));
-      CKR(cudaStreamWaitEvent(h->copy_stream, h->chunk_ev[ci], 0));
-      if (posterior && !direct[0]) CKR(cudaMemcpyAsync(posterior + c0 * n * D, d_post + c0 * n * D, sizeof(double) * nc * n * D, cudaMemcpyDeviceToHost, h->copy_stream));
-      if (stats && !direct[1]) CKR(cudaMemcpyAsync(stats + c0 * n, d_stats + c0 * n, sizeof(dhmc_tree_stats) * nc * n, cudaMemcpyDeviceToHost, h->copy_stream));
-      if (eps_used && !direct[2]) CKR(cudaMemcpyAsync(eps_used + c0 * n, d_eps + c0 * n, sizeof(double) * nc * n, cudaMemcpyDeviceToHost, h->copy_stream));
-      if (logdens && !direct[3]) CKR(cudaMemcpyAsync(logdens + c0 * n, d_ld + c0 * n, sizeof(double) * nc * n, cudaMemcpyDeviceToHost, h->copy_stream));
-      if (h->trace) CKR(cudaEventRecord(h->copy_ev[ci], h->copy_stream));
+      CK(cudaEventRecord(h->chunk_ev[ci], h->stream));
+      CK(cudaStreamWaitEvent(h->copy_stream, h->chunk_ev[ci], 0));
+      for (const Output& o : out)
+        if (o.host && !o.direct) {
+          const size_t at = c0 * n * o.row;
+          CK(cudaMemcpyAsync((char*)o.host + at, (const char*)o.dev + at, nc * n * o.row, cudaMemcpyDeviceToHost, h->copy_stream));
+        }
+      if (h->trace) CK(cudaEventRecord(h->copy_ev[ci], h->copy_stream));
     }
   }
   tr_pt[1] = tr_ms();
   unsigned long long steps = 0;
-  CKR(cudaMemcpyAsync(&steps, h->total_steps, sizeof steps, cudaMemcpyDeviceToHost, h->stream));
-  CKR(cudaStreamSynchronize(h->stream));
+  CK(cudaMemcpyAsync(&steps, h->total_steps, sizeof steps, cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
   tr_pt[2] = tr_ms();
-  CKR(cudaStreamSynchronize(h->copy_stream));
+  CK(cudaStreamSynchronize(h->copy_stream));
   tr_pt[3] = tr_ms();
-  CKS(read_timer(h));
+  if ((rc = read_timer(h)) != DHMC_OK) return rc;
   if (h->trace && nchunks > 1) {
     float t;
     std::fprintf(stderr, "[dhmc trace] chunks %d:", nchunks);
@@ -1286,9 +1225,6 @@ static int run_nuts(dhmc_handle* h, int N, const AdaptConfig& cfg, double lambda
                  tr_pt[0], tr_pt[1], tr_pt[2], tr_pt[3]);
     cudaGetLastError();
   }
-#undef CKR
-#undef CKS
-  cleanup();
   h->last_steps = (int64_t)steps;
   if (advance_t) h->t += (uint32_t)N;
   if (q_host) h->has_position = true;
@@ -1299,21 +1235,16 @@ static int run_nuts(dhmc_handle* h, int N, const AdaptConfig& cfg, double lambda
                                     : "sampling: non-finite position, acceptance rate or step size");
   if (h->trace) std::fprintf(stderr, "[dhmc trace] host: after status check %.2f ms\n", tr_ms());
   if (rc != DHMC_OK) return rc;
-  if (cfg.metric == DHMC_METRIC_DIAGONAL && h->dense) {   // κ ← Diagonal: back to the diagonal kernels
-    h->dense = false; h->pooled = false;
-    rc = plan(h);
-    if (rc != DHMC_OK) return rc;
-  }
+  if (cfg.metric == DHMC_METRIC_DIAGONAL) return set_metric_kind(h, false, false);   // κ ← Diagonal: the diagonal kernels
   if (cfg.metric == DHMC_METRIC_SYMMETRIC) {
     // κ = GaussianKineticEnergy(regularize_M⁻¹(sample_M⁻¹(Symmetric, X), λ)) — mcmc.jl:282
-    const int fgrid = (int)std::min<size_t>((size_t)h->sm_count * 4, (size_t)h->cfg.n_chains);
+    const int fgrid = factor_grid(h);
     if (pool_metric)
       k_cov_pool<<<fgrid, 128, sizeof(double) * h->cfg.dim, h->stream>>>(h->covt, h->mean_pool, h->minv_dense, N, lambda, (int)h->cfg.dim, (int)h->cfg.n_chains);
     else
       k_cov_finish<<<fgrid, 128, 0, h->stream>>>(h->covt, h->minv_dense, N, lambda, (int)h->cfg.dim, (int)h->cfg.n_chains);
     h->launches += 1;
-    h->pooled = pool_metric;
-    rc = factor_and_switch(h);
+    rc = factor_and_switch(h, pool_metric);
   }
   return rc;
 }

@@ -104,8 +104,10 @@ const char* dhmc_last_error(dhmc_handle* h);
 int dhmc_get_layout(dhmc_handle* h, int32_t* threads_per_chain, int32_t* elems_per_thread);
 
 /* ---- problem: replaces the ℓ argument (LogDensityProblems object) ------ */
-/* params: DIAG_NORMAL [mu(D), prec(D)]; LOGISTIC [N, X row-major (N*D), y (N)]; STD_NORMAL / FUNNEL: n == 0;
- * USER: any block of doubles, handed to the user's formulas as `params`. */
+/* params: DIAG_NORMAL [mu(D), prec(D)]; LOGISTIC [N, X row-major (N*D), y (N)] with an integer 1 <= N < 2^31 and
+ * 0 <= y <= 1; STD_NORMAL / FUNNEL: n == 0; USER: any block of doubles, handed to the user's formulas as `params`.
+ * Everything is checked before anything is allocated; on any error the previous problem (one problem or a batch) stays
+ * in effect. */
 int dhmc_set_problem(dhmc_handle* h, const double* params, size_t n);
 /* Problem batch: n_problems posteriors of the handle's family and dimension, each with its own parameter block, on one
  * handle.  Problem p's block is params + p*n_per_problem, in the format of dhmc_set_problem (LOGISTIC: every block has the

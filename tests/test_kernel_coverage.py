@@ -40,8 +40,7 @@ UTILITY_KERNELS = {
     # the window estimate of a Symmetric / pooled Symmetric stage against the exact covariance of the window
     "k_cov_finish": "test_utility_kernels.py::test_window_metric_is_the_regularized_covariance_of_the_window",
     "k_cov_pool": "test_utility_kernels.py::test_window_metric_is_the_regularized_covariance_of_the_window",
-    # the packed logistic cases (8 chains per CTA): padded M⁻¹ blocks (dense phase) and padded rows of X
-    "k_pad_metric": "test_kernel_coverage.py::test_case_matches_oracle",
+    # the packed logistic cases (8 chains per CTA): padded rows of X and padded M⁻¹ blocks (dense phase)
     "k_pad_rows": "test_kernel_coverage.py::test_case_matches_oracle",
     # Xᵀ of every logistic case
     "k_transpose": "test_kernel_coverage.py::test_case_matches_oracle",
@@ -49,10 +48,9 @@ UTILITY_KERNELS = {
     "k_pilot_mean": "test_utility_kernels.py::test_ess_rhat_matches_the_exact_reference",
     "k_ess_rhat": "test_utility_kernels.py::test_ess_rhat_matches_the_exact_reference",
     "k_acceptance_hist": "test_utility_kernels.py::test_acceptance_quantiles_within_one_bin_of_type7",
-    # one diagonal M⁻¹ [D] broadcast to every chain, then trees against the oracle
+    # one diagonal M⁻¹ [D] broadcast to every chain, then trees against the oracle; the broadcast of one Symmetric
+    # M⁻¹ [D, D] (the cases above dim 256) is checked by test_kernel_coverage.py::test_case_matches_oracle
     "k_broadcast": "test_gpu_parity.py::test_one_dimensional_problem",
-    # one Symmetric M⁻¹ [D, D] broadcast to every chain (the cases above dim 256)
-    "k_broadcast_mat": "test_kernel_coverage.py::test_case_matches_oracle",
     # a scalar step size filled into every chain, then trees against the oracle
     "k_fill": "test_gpu_parity.py::test_one_dimensional_problem",
 }
