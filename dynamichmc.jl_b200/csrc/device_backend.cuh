@@ -32,7 +32,7 @@ constexpr int kRedWidth = 8;   // values per cross-warp exchange row
 constexpr int kMaxWarps = 8;   // T <= 256
 
 struct SmemLayout {
-  int red_off;    // doubles: [2][kMaxWarps][kRedWidth]
+  int red_off;    // doubles: [2][kMaxWarps][kRedWidth], or with rg > 1 reduction groups [2][W][rg · kRedWidth]
   int ctl_off;    // bytes from base: Entry[W][levels]
   int misc_off;   // bytes: int[4]
   int top_off;    // bytes: TopState[W] (transition-level scalars, one copy per warp)
@@ -43,13 +43,16 @@ struct SmemLayout {
 };
 // stride = doubles per slot (a slot of the dense metric holds a (p, p♯) pair), xs = doubles of staging
 // levels = stack entries per warp (max_depth + 1), ntab = entries of the slot-address table (>= n_slots); kernels for
-// max_depth <= 12 use the compile-time standard values
+// max_depth <= 12 use the compile-time standard values.  rg = groups of kRedWidth values that one all-reduce carries
+// (DeviceBackend::kFused: the leapfrog's sums and every merge check of a leaf)
 constexpr int kStdLevels = 13, kStdTab = 64;
-__host__ __device__ inline SmemLayout smem_layout(int W, int n_sm, size_t stride, size_t xs = 0, int levels = kStdLevels, int ntab = kStdTab) {
+__host__ __device__ inline size_t red_half_doubles(int W, int rg) { return rg > 1 ? (size_t)W * kRedWidth * rg : (size_t)kMaxWarps * kRedWidth; }
+__host__ __device__ inline SmemLayout smem_layout(int W, int n_sm, size_t stride, size_t xs = 0, int levels = kStdLevels, int ntab = kStdTab,
+                                                  int rg = 1) {
   SmemLayout L;
   size_t off = 0;
   L.red_off = 0;
-  off += sizeof(double) * 2 * kMaxWarps * kRedWidth;
+  off += sizeof(double) * 2 * red_half_doubles(W, rg);
   L.ctl_off = (int)off;
   off += sizeof(Entry) * (size_t)W * (size_t)levels;
   off = (off + 15) & ~(size_t)15;
@@ -636,8 +639,22 @@ struct DeviceBackend {
       w[0] = w[0] + __shfl_xor_sync(0xffffffffu, w[0], OFF);
     }
   }
+  // the pairwise tree over the warps' partials b[0], b[S], b[2S], … (offsets 32, 64, … of the canonical order)
+  template <int S>
+  __device__ __forceinline__ static double warp_sum(const double* b) { return warp_sum(b, S); }
+  __device__ __forceinline__ static double warp_sum(const double* b, int S) {
+    if (W == 1) return b[0];
+    if (W == 2) return b[0] + b[S];
+    if (W == 4) return (b[0] + b[S]) + (b[2 * S] + b[3 * S]);
+    return ((b[0] + b[S]) + (b[2 * S] + b[3 * S])) + ((b[4 * S] + b[5 * S]) + (b[6 * S] + b[7 * S]));
+  }
+  __device__ __forceinline__ int red_half() const {
+    if constexpr (kFused) return red_half_n;
+    else return kMaxWarps * kRedWidth;
+  }
+  // the intra-warp part: returns which of the N values this lane ends up with (its warp's partial in *out)
   template <int N>
-  __device__ __forceinline__ void reduce(double (&v)[N]) {
+  __device__ __forceinline__ int warp_scatter(const double (&v)[N], double* out) const {
     constexpr int P = N <= 1 ? 1 : N <= 2 ? 2 : N <= 4 ? 4 : 8;
     static_assert(N <= kRedWidth, "at most 8 values per reduction");
     double w[P];
@@ -649,25 +666,137 @@ struct DeviceBackend {
     rs_stage<(P >= 4 ? P / 4 : 1), 4>(w, idx);
     rs_stage<1, 2>(w, idx);
     rs_stage<1, 1>(w, idx);
-    double* buf = red + red_buf * (kMaxWarps * kRedWidth);
+    *out = w[0];
+    return idx;
+  }
+  template <int N>
+  __device__ __forceinline__ void reduce(double (&v)[N]) {
+#if defined(DHMC_PHASE_CLOCKS)
+    const bool ph_leaf_red = ph_cur == kPhLfElem || ph_cur == kPhMcElem;   // the reductions of a leaf are profiled
+    if (ph_leaf_red) phase_mark(ph_cur + 1);
+#endif
+    double w0;
+    const int idx = warp_scatter(v, &w0);
+    double* buf = red + red_buf * red_half();
     red_buf ^= 1;
-    buf[warp * kRedWidth + idx] = w[0];
+    buf[warp * kRedWidth + idx] = w0;
     group_sync();
 #pragma unroll
-    for (int n = 0; n < N; ++n) {
-      const double* b = buf + n;
-      if (W == 1) {
-        v[n] = b[0];
-      } else if (W == 2) {
-        v[n] = b[0] + b[kRedWidth];
-      } else if (W == 4) {
-        v[n] = (b[0] + b[kRedWidth]) + (b[2 * kRedWidth] + b[3 * kRedWidth]);
-      } else {
-        v[n] = ((b[0] + b[kRedWidth]) + (b[2 * kRedWidth] + b[3 * kRedWidth])) +
-               ((b[4 * kRedWidth] + b[5 * kRedWidth]) + (b[6 * kRedWidth] + b[7 * kRedWidth]));
+    for (int n = 0; n < N; ++n) v[n] = warp_sum<kRedWidth>(buf + n);
+#if defined(DHMC_PHASE_CLOCKS)
+    if (ph_leaf_red) phase_mark(kPhCtrl);
+#endif
+  }
+
+  // ---- one all-reduce per leaf (diagonal metric, one chain per CTA).  The machine tells leapfrog() which merges the new
+  // leaf may need: its ctz(k) stack merges (top entry first) and, on the last leaf of an adjacent tree, the doubling-level
+  // check against the whole tree.  Their dot products depend only on the new p and on slots fixed before the leaf, so the
+  // leapfrog computes them all right after its own elementwise pass (ρ chained speculatively, as merge_check would) and
+  // ONE all-reduce carries everything: group 0 = the leapfrog's sums plus the leaf-leaf merge's two products in columns
+  // kLeafCol, kLeafCol + 1; group j + (no stack merge ? 1 : 0) = the six products of merge j.  merge_check(j, …) then only
+  // reads the sums; those of merges the control never reaches are dropped.  Every value keeps its per-thread order and
+  // its pairwise tree (warp_scatter / warp_sum), so the sums are those of one merge_check at a time.  User models keep
+  // one reduction per check: with the merges inlined behind their model code the C2-shaped user kernel ran slower.
+  static constexpr bool kFused = !DENSE && PACK == 1 && FAM != DHMC_FAMILY_USER;
+  static constexpr bool kLeafMerges = true;   // the interface (nuts_machine.cuh); kernels without kFused check one merge at a time
+  static constexpr int kLeafCol = 6;
+  int red_half_n, red_row;                  // kFused: doubles per buffer half / per warp row (rg · kRedWidth)
+  int m_sp, m_c, m_dbl;                     // merges of the current leaf: stack height, stack merges, doubling check
+  int m_shift;                              // group of merge j = j + m_shift
+  const double* m_buf;                      // the buffer half that holds their sums
+
+  template <int N>
+  __device__ __forceinline__ void reduce_leaf(double (&v)[N]) {
+    if constexpr (kFused) {
+      if (m_c > 0 || m_dbl) { reduce_fused(v); return; }
+    }
+    reduce(v);
+  }
+  template <int N>
+  __device__ __forceinline__ void reduce_fused(double (&v)[N]) {
+    static_assert(N <= kLeafCol, "group 0 holds the leapfrog's sums and two merge products");
+    DHMC_PHASE(*this, kPhMcElem);
+    double* buf = red + red_buf * red_half_n;
+    red_buf ^= 1;
+    double* row = buf + warp * red_row;
+    {
+      double g0[kRedWidth];
+#pragma unroll
+      for (int n = 0; n < kLeafCol; ++n) g0[n] = n < N ? v[n] : 0.0;
+      g0[kLeafCol] = 0.0; g0[kLeafCol + 1] = 0.0;
+      if (m_c > 0) {                        // merge 0: two single leaves (see merge_check)
+        const double* pEf = slot(ctl[m_sp - 1].sfirst);
+#pragma unroll
+        for (int e = 0; e < EPL; ++e) {
+          const double Ef = pEf[e * T];
+          const double A = Ef + p[e];
+          const double mEf = minv[e] * Ef, mLl = minv[e] * p[e];
+          g0[kLeafCol] = g0[kLeafCol] + mEf * A;
+          g0[kLeafCol + 1] = g0[kLeafCol + 1] + mLl * A;
+          rhoL[e] = A;
+        }
       }
+      double w0;
+      const int idx = warp_scatter(g0, &w0);
+      row[idx] = w0;
+    }
+    m_shift = m_c > 0 ? 0 : 1;
+    const int nm = m_c + m_dbl;
+    for (int j = 1 - m_shift; j < nm; ++j) {
+      int sEf, sEl, sEr, sLf;
+      bool lleaf = false;
+      if (j < m_c) {                        // stack merge j: E = the entry below, L = the subtree of merges 0…j-1
+        const Entry& E = ctl[m_sp - 1 - j];
+        sEf = E.sfirst; sEl = E.slast; sEr = E.srho;
+        sLf = ctl[m_sp - j].sfirst;
+      } else {                              // the doubling check: E = the whole tree so far, L = this adjacent tree
+        const TopState& S = top();
+        sEf = S.s_op; sEl = S.s_near; sEr = S.s_rhot;
+        lleaf = m_c == 0;
+        sLf = lleaf ? sEf : ctl[m_sp - m_c].sfirst;
+      }
+      const double* pEf = slot(sEf);
+      const double* pEl = slot(sEl);
+      const double* pEr = slot(sEr);
+      const double* pLf = slot(sLf);
+      double d[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+#pragma unroll
+      for (int e = 0; e < EPL; ++e) {
+        const double Ef = pEf[e * T], El = pEl[e * T], Er = pEr[e * T];
+        const double Lf = lleaf ? p[e] : pLf[e * T];
+        const double Lr = lleaf ? p[e] : rhoL[e];
+        const double A = Er + Lf, Bv = El + Lr, R = Er + Lr;
+        const double mEf = minv[e] * Ef, mLf = minv[e] * Lf, mEl = minv[e] * El, mLl = minv[e] * p[e];
+        d[0] = d[0] + mEf * A;  d[1] = d[1] + mLf * A;
+        d[2] = d[2] + mEl * Bv; d[3] = d[3] + mLl * Bv;
+        d[4] = d[4] + mEf * R;  d[5] = d[5] + mLl * R;
+        rhoL[e] = R;
+      }
+      double w0;
+      const int idx = warp_scatter(d, &w0);
+      row[(j + m_shift) * kRedWidth + idx] = w0;
+    }
+    DHMC_PHASE(*this, kPhLfRed);
+    group_sync();
+#pragma unroll
+    for (int n = 0; n < N; ++n) v[n] = warp_sum(buf + n, red_row);
+    m_buf = buf;
+    DHMC_PHASE(*this, kPhCtrl);
+  }
+
+#if defined(DHMC_PHASE_CLOCKS)
+  unsigned long long* ph_acc;               // this CTA's kPhCount counters
+  long long ph_t;                           // clock64() at the last mark
+  int ph_cur;                               // the phase that time since the last mark belongs to
+  __device__ __forceinline__ void phase_mark(int ph) {
+    if (ctid == 0) {
+      const long long t = clock64();
+      atomicAdd(ph_acc + ph_cur, (unsigned long long)(t - ph_t));
+      ph_t = t; ph_cur = ph;
     }
   }
+  __device__ __forceinline__ void phase_leaf() { if (ctid == 0) atomicAdd(ph_acc + kPhLeaves, 1ull); }
+#endif
 
   // ---- lane-parallel scalar math: all threads of a chain hold the same scalars,
   // so independent transcendental evaluations are spread over lanes and shared
@@ -1125,7 +1254,7 @@ struct DeviceBackend {
           }
         }
       }
-      reduce(r);
+      reduce_leaf(r);
       double l = dhmc_logit_lq(r[0], r[1]);
       if (!((dm_isfinite(l) && r[3] == 0.0) || l == -dm_inf())) *flags |= 4;
       l = sanitise(l, r[3] != 0.0);
@@ -1166,7 +1295,7 @@ struct DeviceBackend {
           }
         }
       }
-      reduce(r2);
+      reduce_leaf(r2);
       double l = dhmc_funnel_lq(v, ev, S, D);
       if (!((dm_isfinite(l) && r2[1] == 0.0) || l == -dm_inf())) *flags |= 4;
       l = sanitise(l, r2[1] != 0.0);
@@ -1200,7 +1329,7 @@ struct DeviceBackend {
           }
         }
       }
-      reduce(r);
+      reduce_leaf(r);
       double l = (FAM == DHMC_FAMILY_STD_NORMAL) ? dhmc_std_lq(r[0]) : dhmc_diag_lq(r[0]);
       if (!((dm_isfinite(l) && r[3] == 0.0) || l == -dm_inf())) *flags |= 4;
       l = sanitise(l, r[3] != 0.0);
@@ -1212,7 +1341,10 @@ struct DeviceBackend {
   }
 
   // leapfrog(H, z, ϵ) — hamiltonian.jl:273-282, then logdensity(H, z′).
-  __device__ __forceinline__ double leapfrog(double eps, int* flags) {
+  // sp, nc, dbl: the merges the new leaf may need (see reduce_fused); dense and packed backends check them one at a time
+  __device__ __forceinline__ double leapfrog(double eps, int* flags, int sp = 0, int nc = 0, bool dbl = false) {
+    DHMC_PHASE(*this, kPhLfElem);
+    if constexpr (kFused) { m_sp = sp; m_c = nc; m_dbl = dbl ? 1 : 0; }
     tid = pin(tid); lane = pin(lane); warp = pin(warp); mparams = pin(mparams);
     const double h = eps / 2;
     double qbad = 0.0;
@@ -1242,13 +1374,26 @@ struct DeviceBackend {
       }
       double ksum;
       eval_model(true, h, qbad, &ksum, flags);  // Q′ = evaluate_ℓ; p′ = pₘ + ϵ/2 ∇ℓq′  :279-280
+      if constexpr (kFused) { m_c = 0; m_dbl = 0; }
       return hamiltonian_logdensity(lq, ksum);
     }
   }
 
   // The six dot products of combine_turn_statistics (NUTS.jl:130-139) in build
   // order; leaves the combined ρ in rhoL.  Returns true when turning.
-  __device__ __forceinline__ bool merge_check(int sEf, int sEl, int sEr, int sLf, bool L_leaf) {
+  // j: the merge's place among those of the current leaf (reduce_fused).
+  __device__ __forceinline__ bool merge_check(int j, int sEf, int sEl, int sEr, int sLf, bool L_leaf) {
+    if constexpr (kFused) {                 // the sums came with the leapfrog's all-reduce
+      const int g = j + m_shift;
+      if (g == 0)
+        return warp_sum(m_buf + kLeafCol, red_row) < 0 || warp_sum(m_buf + kLeafCol + 1, red_row) < 0;
+      const double* bg = m_buf + g * kRedWidth;
+      double d[6];
+#pragma unroll
+      for (int n = 0; n < 6; ++n) d[n] = warp_sum(bg + n, red_row);
+      return d[0] < 0 || d[1] < 0 || d[2] < 0 || d[3] < 0 || d[4] < 0 || d[5] < 0;
+    }
+    DHMC_PHASE(*this, kPhMcElem);
     if constexpr (DENSE) {
       // p♯ of the four edge momenta come from the slots (stored next to p); ρ slots hold ρ only
       const double* pEf = slot(sEf);

@@ -331,6 +331,9 @@ struct dhmc_handle {
   double* mparams = nullptr;
   int* status = nullptr;
   double* scratch = nullptr;
+#if defined(DHMC_PHASE_CLOCKS)
+  unsigned long long* phase_clocks = nullptr;   // leaf profile: kPhCount counters for each of up to 32 CTAs per SM
+#endif
   unsigned* counter = nullptr;
   unsigned long long* total_steps = nullptr;
   uint32_t t = 0;
@@ -395,6 +398,12 @@ static size_t lr_rows(const dhmc_handle* h) {
   return std::max<size_t>(h->G > 1 ? 0 : (size_t)h->grid, (size_t)h->light_grid);
 }
 
+// groups of the persistent kernels' reduction buffer (DeviceBackend::kFused): the last leaf of a depth-d adjacent tree carries
+// d stack merges and the doubling check, the first two in group 0, so max_depth groups (two at max_depth 1)
+static int red_groups(const dhmc_handle* h) {
+  return !h->dense && h->G == 1 && h->cfg.family != DHMC_FAMILY_USER ? std::max(2, h->cfg.max_depth) : 1;
+}
+
 // Plan the persistent kernels for the current metric kind: CTAs per SM (register
 // limited), how many slots fit in shared memory, and the global scratch arena.
 static int plan(dhmc_handle* h) {
@@ -406,7 +415,7 @@ static int plan(dhmc_handle* h) {
   const int G = h->G;
   auto heavy_smem = [&](int n_sm) -> size_t {
     return G > 1 ? (size_t)G * group_smem_bytes(h->W, n_sm, slot_doubles, xs, h->levels, h->ntab) + tma_smem_bytes(G, (int)h->cfg.dim)
-                 : smem_layout(h->W, n_sm, slot_doubles, xs, h->levels, h->ntab).total;
+                 : smem_layout(h->W, n_sm, slot_doubles, xs, h->levels, h->ntab, red_groups(h)).total;
   };
   struct { size_t total; } L0{heavy_smem(0)};
   h->smem_light = smem_layout(h->W, 0, slot_doubles, xs).total;      // light kernels: standard layout
@@ -461,8 +470,12 @@ static KArgs base_args(dhmc_handle* h) {
   a.max_depth = h->cfg.max_depth; a.min_delta = h->cfg.min_delta;
   a.t0 = h->t;
   a.scratch = h->scratch; a.scratch_per_cta = h->scratch_per_cta;
+#if defined(DHMC_PHASE_CLOCKS)
+  a.phase_clocks = h->phase_clocks;
+#endif
   a.n_sm = h->n_sm; a.n_slots = h->n_slots; a.stride = h->stride * (h->dense ? 2 : 1);
   a.levels = h->levels; a.ntab = h->ntab;
+  a.red_groups = red_groups(h);
   a.counter = h->counter; a.total_steps = h->total_steps;
   a.chain_begin = 0; a.chain_end = (int)h->cfg.n_chains;
   a.minv_dense = h->minv_dense; a.wt = h->wt; a.covt = nullptr; a.minv_pad = h->minv_pad; a.mean_out = nullptr; a.pooled = h->pooled ? 1 : 0;
@@ -484,7 +497,7 @@ static int read_timer(dhmc_handle* h) {
 // before and right after the kernel, so that they time it alone.  reset_steps: zero the Σ steps counter first.
 static int launch(dhmc_handle* h, KernelId k, KArgs a, cudaEvent_t before, cudaEvent_t after, bool reset_steps = true) {
   const bool heavy = (k == K_NUTS || k == K_SEARCH);
-  if (!heavy) { a.n_sm = 0; }
+  if (!heavy) { a.n_sm = 0; a.red_groups = 1; }
   const size_t smem = heavy ? h->smem_bytes : smem_layout(h->W, 0, a.stride, (size_t)a.xs_doubles).total;
   int grid = heavy ? h->grid : h->light_grid;
   const int G = heavy ? h->G : 1;
@@ -572,6 +585,9 @@ int dhmc_destroy(dhmc_handle* h) {
   cudaSetDevice(h->cfg.device);
   cudaFree(h->q); cudaFree(h->g); cudaFree(h->lq); cudaFree(h->p); cudaFree(h->minv); cudaFree(h->eps);
   cudaFree(h->mparams); cudaFree(h->status); cudaFree(h->scratch); cudaFree(h->counter);
+#if defined(DHMC_PHASE_CLOCKS)
+  cudaFree(h->phase_clocks);
+#endif
   cudaFree(h->total_steps);
   cudaFree(h->minv_dense); cudaFree(h->wt); cudaFree(h->covt); cudaFree(h->dense_tmp); cudaFree(h->minv_pad); cudaFree(h->mean_pool);
   cudaFree(h->lX); cudaFree(h->lXt); cudaFree(h->ly); cudaFree(h->lr); cudaFree(h->lXp); cudaFree(h->problems);
@@ -642,6 +658,10 @@ int dhmc_create(const dhmc_config* cfg, dhmc_handle** out) {
   cudaDeviceProp prop;
   CKC(cudaGetDeviceProperties(&prop, cfg->device));
   h->sm_count = prop.multiProcessorCount;
+#if defined(DHMC_PHASE_CLOCKS)
+  CKC(cudaMalloc(&h->phase_clocks, sizeof(unsigned long long) * kPhCount * 32 * (size_t)h->sm_count));
+  CKC(cudaMemset(h->phase_clocks, 0, sizeof(unsigned long long) * kPhCount * 32 * (size_t)h->sm_count));
+#endif
   CKC(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
   CKC(cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking));
   CKC(cudaStreamCreateWithFlags(&h->h2d_stream, cudaStreamNonBlocking));
@@ -1490,6 +1510,21 @@ int dhmc_acceptance_quantiles_dev(dhmc_handle* h, const dhmc_tree_stats* stats_d
 int dhmc_last_total_steps(dhmc_handle* h, int64_t* steps) { if (!h || !steps) return DHMC_EARG; *steps = h->last_steps; return DHMC_OK; }
 int dhmc_last_kernel_ms(dhmc_handle* h, double* ms) { if (!h || !ms) return DHMC_EARG; *ms = h->last_ms; return DHMC_OK; }
 int dhmc_kernel_launches(dhmc_handle* h, int64_t* n) { if (!h || !n) return DHMC_EARG; *n = h->launches; return DHMC_OK; }
+#if defined(DHMC_PHASE_CLOCKS)
+// Leaf profile of the diagnostic build (benchmarks/leaf_phases.py): out[kPhCount] = the counters summed over all CTAs since the
+// last reset (clock cycles of thread 0 of each CTA per phase, and the number of leaves); reset != 0 zeroes them afterwards.
+int dhmc_phase_clocks(dhmc_handle* h, uint64_t* out, int reset) {
+  if (!h || !out) return DHMC_EARG;
+  const size_t n = (size_t)kPhCount * 32 * (size_t)h->sm_count;
+  std::vector<unsigned long long> v(n);
+  CK(cudaDeviceSynchronize());
+  CK(cudaMemcpy(v.data(), h->phase_clocks, sizeof(unsigned long long) * n, cudaMemcpyDeviceToHost));
+  for (int k = 0; k < kPhCount; ++k) out[k] = 0;
+  for (size_t i = 0; i < n; ++i) out[i % kPhCount] += v[i];
+  if (reset) CK(cudaMemset(h->phase_clocks, 0, sizeof(unsigned long long) * n));
+  return DHMC_OK;
+}
+#endif
 
 // ---- multi-GPU (SURVEY §8e): chains are sharded over ranks with no data-path collective; the one exchange is the
 // all-gather of (thinned) draws / final positions at the end.  One process per GPU; rank 0 creates the id, the host

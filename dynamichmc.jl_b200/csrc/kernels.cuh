@@ -78,6 +78,10 @@ struct KArgs {
   // the problem index is a 32-bit division.
   int batch_k;
   const ProblemDesc* problems;
+  int red_groups;               // groups of the reduction buffer (smem_layout rg) of the kernels with DeviceBackend::kFused
+#if defined(DHMC_PHASE_CLOCKS)
+  unsigned long long* phase_clocks;   // leaf profile: kPhCount counters per CTA (nuts_machine.cuh)
+#endif
 };
 
 // Register budget: minimum resident CTAs per SM the compiler must allow for.
@@ -98,7 +102,9 @@ __device__ __forceinline__ void setup_backend(DeviceBackend<EPL, FAM, W, DN, G, 
   b.ctid = threadIdx.x; b.grp = 0;
   b.tid = threadIdx.x; b.lane = threadIdx.x & 31; b.warp = threadIdx.x >> 5;
   b.D = a.D;
-  const SmemLayout L = smem_layout(W, a.n_sm, b.stride, (size_t)a.xs_doubles, DP ? a.levels : kStdLevels, DP ? a.ntab : kStdTab);
+  using Bk = DeviceBackend<EPL, FAM, W, DN, G, DP>;
+  const int rg = Bk::kFused ? a.red_groups : 1;
+  const SmemLayout L = smem_layout(W, a.n_sm, b.stride, (size_t)a.xs_doubles, DP ? a.levels : kStdLevels, DP ? a.ntab : kStdTab, rg);
   b.lX = a.lX; b.lXt = a.lXt; b.ly = a.ly; b.lN = a.lN; b.lLd = a.lLd;
   b.lr = a.lr ? a.lr + (size_t)blockIdx.x * a.lN : nullptr;
   b.cb_beta = b.cb_grad = nullptr;
@@ -130,6 +136,10 @@ __device__ __forceinline__ void setup_backend(DeviceBackend<EPL, FAM, W, DN, G, 
   b.Mrow = nullptr; b.Wt = nullptr; b.covt = nullptr;
   b.red = reinterpret_cast<double*>(smem + L.red_off);
   b.red_buf = 0;
+  if constexpr (Bk::kFused) {
+    b.red_half_n = (int)red_half_doubles(W, rg); b.red_row = kRedWidth * rg;
+    b.m_sp = 0; b.m_c = 0; b.m_dbl = 0; b.m_shift = 0; b.m_buf = b.red;
+  }
   b.rexp_cache = 0.0; b.rexp_base = 0xffffffffu; b.rexp_t = 0xffffffffu;
   b.ctl = reinterpret_cast<Entry*>(smem + L.ctl_off) + b.warp * (DP ? a.levels : kStdLevels);
   b.tops = reinterpret_cast<TopState*>(smem + L.top_off + b.warp * ((sizeof(TopState) + 15) & ~(size_t)15));
@@ -139,6 +149,10 @@ __device__ __forceinline__ void setup_backend(DeviceBackend<EPL, FAM, W, DN, G, 
   b.slot_tab = reinterpret_cast<double**>(smem + L.tab_off); b.n_tab = DP ? a.ntab : kStdTab;
   b.build_slot_table();
   b.mparams = a.mparams;
+#if defined(DHMC_PHASE_CLOCKS)
+  b.ph_acc = a.phase_clocks + (size_t)blockIdx.x * kPhCount;
+  b.ph_t = clock64(); b.ph_cur = kPhTrans;
+#endif
 }
 
 // packed groups: every warp draws its own chains
@@ -246,7 +260,7 @@ __global__ void __launch_bounds__(32 * W * G, G > 1 ? 1 : min_ctas(W, EPL)) k_nu
   DeviceBackend<EPL, FAM, W, DN, G, DP> b;
   setup_backend(b, a, smem);
   int* s_misc = reinterpret_cast<int*>(smem + smem_layout(W, a.n_sm, b.stride, (size_t)a.xs_doubles, DP ? a.levels : kStdLevels,
-                                                          DP ? a.ntab : kStdTab).misc_off);   // one chain per CTA: the queue's broadcast slot
+                                                          DP ? a.ntab : kStdTab, decltype(b)::kFused ? a.red_groups : 1).misc_off);   // one chain per CTA: the queue's broadcast slot
   for (;;) {
     int c;
     if constexpr (G > 1) {
@@ -289,7 +303,7 @@ __global__ void __launch_bounds__(32 * W * G, G > 1 ? 1 : min_ctas(W, EPL)) k_se
   DeviceBackend<EPL, FAM, W, DN, G, DP> b;
   setup_backend(b, a, smem);
   int* s_misc = reinterpret_cast<int*>(smem + smem_layout(W, a.n_sm, b.stride, (size_t)a.xs_doubles, DP ? a.levels : kStdLevels,
-                                                          DP ? a.ntab : kStdTab).misc_off);   // one chain per CTA: the queue's broadcast slot
+                                                          DP ? a.ntab : kStdTab, decltype(b)::kFused ? a.red_groups : 1).misc_off);   // one chain per CTA: the queue's broadcast slot
   for (;;) {
     int c;
     if constexpr (G > 1) {

@@ -38,6 +38,8 @@
 #include "../../include/dhmc.h"
 #include "../../include/dhmc_math.h"
 
+#include <type_traits>
+
 #if defined(__CUDACC__)
 #define DHMC_M __device__ __forceinline__
 #define DHMC_COLD __device__ __noinline__      // rarely taken paths: kept out of line so that they cost the hot loop no registers
@@ -47,6 +49,34 @@
 #endif
 
 namespace dhmc {
+
+// Leaf profile (diagnostic builds with -DDHMC_PHASE_CLOCKS only, benchmarks/leaf_phases.py): thread 0 of each CTA attributes
+// the clock64() time between two marks to the phase the first mark named.  Without the switch the marks compile to nothing.
+enum : int {
+  kPhLfElem,    // the leapfrog's elementwise pass (model, momentum, partial sums)
+  kPhLfRed,     // the leapfrog's all-reduce
+  kPhMcElem,    // merge checks: slot loads and dot-product arithmetic
+  kPhMcRed,     // merge checks: all-reduce
+  kPhCtrl,      // scalar control of the tree (Δ, logaddexp, randexp, slot bookkeeping)
+  kPhPush,      // stack pushes: slot stores
+  kPhTrans,     // transition level: momentum draw, doubling bookkeeping, draw output
+  kPhLeaves,    // (a count, not a time: leaves built)
+  kPhCount
+};
+#if defined(DHMC_PHASE_CLOCKS)
+#define DHMC_PHASE(be, ph) (be).phase_mark(ph)
+#define DHMC_PHASE_LEAF(be) (be).phase_leaf()
+#else
+#define DHMC_PHASE(be, ph) ((void)0)
+#define DHMC_PHASE_LEAF(be) ((void)0)
+#endif
+
+// A backend with `kLeafMerges = true` is told, when it leapfrogs, which merges the new leaf may need (leapfrog(ε, flags,
+// stack height, ctz(k), last leaf?)) and is asked for them by their place among the leaf's merges (merge_check(j, …)), so
+// that it can evaluate them together with the leapfrog (DeviceBackend, one all-reduce per leaf).  Any other backend gets
+// leapfrog(ε, flags) and merge_check(…) one merge at a time.
+template <class B, class = void> struct LeafMerges : std::false_type {};
+template <class B> struct LeafMerges<B, std::void_t<decltype(B::kLeafMerges)>> : std::bool_constant<B::kLeafMerges> {};
 
 constexpr int kMaxLevels = 32;   // max_depth <= MAX_DIRECTIONS_DEPTH = 32 (trees.jl:10, NUTS.jl:190)
 constexpr int kMaskWords = 3;    // slot free-list: 64 slots in a register word + two spill words (max_depth > 12 needs up to 164 slots)
@@ -128,6 +158,24 @@ struct NutsMachine {
     int s = 63;
     while (!((m >> s) & 1ull)) --s;
     return s;
+#endif
+  }
+  static constexpr bool kLeafMerges = LeafMerges<B>::value;
+  DHMC_M double leaf_leapfrog(double eps, int* flags, int sp, unsigned k, unsigned nleaves) {
+    if constexpr (kLeafMerges) return b.leapfrog(eps, flags, sp, ctz(k), k == nleaves);
+    else return b.leapfrog(eps, flags);
+  }
+  DHMC_M bool merge(int j, int sEf, int sEl, int sEr, int sLf, bool L_leaf) {
+    if constexpr (kLeafMerges) return b.merge_check(j, sEf, sEl, sEr, sLf, L_leaf);
+    else return b.merge_check(sEf, sEl, sEr, sLf, L_leaf);
+  }
+  DHMC_M static int ctz(unsigned k) {          // k != 0
+#if defined(__CUDA_ARCH__)
+    return __ffs((int)k) - 1;
+#else
+    int c = 0;
+    while (!((k >> c) & 1u)) ++c;
+    return c;
 #endif
   }
   DHMC_M void init_pool() {
@@ -225,6 +273,7 @@ struct NutsMachine {
   // meaningless (the caller keeps the chain's stored state).
   DHMC_M void transition(uint32_t t_, double eps, const double* p_override,
                           const uint32_t* dir_override, dhmc_tree_stats* ts) {
+    DHMC_PHASE(b, kPhTrans);
     t = t_;
     n_exp = 0;
     // p = rand_p(rng, κ) first, directions second — NUTS.jl:233
@@ -287,12 +336,16 @@ struct NutsMachine {
       int L_vsteps = 0, L_ifirst = 0, L_sfirst = -1, L_szq = -1, L_szg = -1;
       bool L_leaf = true;
       for (unsigned k = 1; k <= nleaves; ++k) {
+        DHMC_PHASE(b, kPhCtrl);
+        DHMC_PHASE_LEAF(b);
         if (!dm_isfinite(b.cur_lq())) {                   // @argcheck isfinite(Q.ℓq), hamiltonian.jl:276
           status |= DHMC_CHAIN_LEAPFROG_NONFINITE;
           break;
         }
         int lf_flags = 0;
-        const double Hn = b.leapfrog(eps_s, &lf_flags);   // move + logdensity(H, z′)
+        // move + logdensity(H, z′); the backend may compute the dot products of the leaf's merges (the ctz(k) stack merges,
+        // then on the last leaf the doubling-level check) alongside: their operands are fixed once p′ is
+        const double Hn = leaf_leapfrog(eps_s, &lf_flags, sp, k, nleaves);
         if (lf_flags & 1) status |= DHMC_CHAIN_NONFINITE_Q;
         pos += fwd ? 1 : -1;
         const double delta = Hn - pi0;                    // NUTS.jl:150
@@ -305,15 +358,10 @@ struct NutsMachine {
           L_omega = delta; L_vlog = leaf_vlog; L_vsteps = 1; L_ifirst = pos;
           L_zlq = b.cur_lq(); L_zH = Hn; L_szq = -1; L_szg = -1; L_sfirst = -1; L_leaf = true;
           b.rho_from_p();
-#if defined(__CUDA_ARCH__)
-          const int c = __ffs((int)k) - 1;                // ctz(k): merges after this leaf
-#else
-          int c = 0;
-          while (!((k >> c) & 1u)) ++c;                   // ctz(k): merges after this leaf
-#endif
+          const int c = ctz(k);                           // merges after this leaf
           for (int j = 0; j < c; ++j) {
             const Entry& E = b.get_entry(--sp);
-            const bool turning = b.merge_check(E.sfirst, E.slast, E.srho, L_sfirst, L_leaf);
+            const bool turning = merge(j, E.sfirst, E.slast, E.srho, L_sfirst, L_leaf);
             // v = combine_visited_statistics(v₋, v₊) precedes the checks, trees.jl:249
             // (ω of the merged tree is computed alongside: two independent logaddexp,
             //  evaluated lane-parallel on the GPU)
@@ -353,12 +401,15 @@ struct NutsMachine {
           break;
         }
         if (k < nleaves) {
-          // push L: materialise what still lives in registers
+          // push L: materialise what still lives in registers.  Slots by role: what merge_check reads on later leaves
+          // (momenta, ρ) comes from the low end of the pool, i.e. shared memory; a proposal's q and ∇ℓ, read at most once
+          // per transition, from the high end, i.e. the global arena whenever the pool outgrows shared memory.
+          DHMC_PHASE(b, kPhPush);
           Entry N;
           N.omega = L_omega; N.vlog = L_vlog; N.vsteps = L_vsteps; N.ifirst = L_ifirst;
           N.zlq = L_zlq; N.zH = L_zH;
           if (L_leaf) {
-            const int sq = alloc_lo(), sg = alloc_lo(), spp = alloc_lo();
+            const int sq = alloc_hi(), sg = alloc_hi(), spp = alloc_lo();
             b.st_q(sq); b.st_g(sg); b.st_p(spp);
             N.szq = (short)sq; N.szg = (short)sg;
             N.sfirst = N.slast = N.srho = (short)spp; N.leaf = 1;
@@ -366,13 +417,14 @@ struct NutsMachine {
             const int sl = alloc_lo(), sr = alloc_lo();
             b.st_p(sl); b.st_rho(sr);
             if (L_szq < 0) {
-              L_szq = alloc_lo(); L_szg = alloc_lo();
+              L_szq = alloc_hi(); L_szg = alloc_hi();
               b.st_q(L_szq); b.st_g(L_szg);
             }
             N.szq = (short)L_szq; N.szg = (short)L_szg;
             N.sfirst = (short)L_sfirst; N.slast = (short)sl; N.srho = (short)sr; N.leaf = 0;
           }
           b.put_entry(sp++, N);
+          DHMC_PHASE(b, kPhCtrl);
         } else {
           vacc_log = L_vlog; vacc_steps = L_vsteps;
         }
@@ -404,7 +456,7 @@ struct NutsMachine {
       depth += 1;                                         // trees.jl:312
       // τ = combine_turn_statistics_in_direction(τ, τ′): the tree so far is the
       // earlier entry with first = far-edge p, last = near-edge p before this subtree
-      const bool turning = b.merge_check(s_op, s_near, s_rhot, L_sfirst, L_leaf);
+      const bool turning = merge(depth - 1, s_op, s_near, s_rhot, L_sfirst, L_leaf);   // the last leaf's merge after its ctz = depth - 1
       if (!L_leaf) release(L_sfirst);
       if (turning) {                                      // trees.jl:316
         term_l = regs_fwd ? i_far : i_near;
@@ -413,7 +465,9 @@ struct NutsMachine {
       }
       b.rho_commit();
       b.st_rho(s_rhot);
+      DHMC_PHASE(b, kPhTrans);
     }
+    DHMC_PHASE(b, kPhTrans);
 
     // TreeStatisticsNUTS — NUTS.jl:238-239
     ts->pi = zt_H;
@@ -480,6 +534,7 @@ struct NutsMachine {
       if (cfg.metric != DHMC_METRIC_NOTHING) b.metric_push(cfg.metric, n + 1);
     }
     if (cfg.metric != DHMC_METRIC_NOTHING) b.metric_finish(cfg.metric, N);   // sample_M⁻¹, mcmc.jl:209-211
+    DHMC_PHASE(b, kPhTrans);
     steps_out = S.total_steps;
     return cfg.adapt ? dm_exp(S.da_logepsbar) : eps;             // final_ϵ :170
   }
