@@ -801,10 +801,15 @@ struct DeviceBackend {
   // ---- lane-parallel scalar math: all threads of a chain hold the same scalars,
   // so independent transcendental evaluations are spread over lanes and shared
   // by shuffle instead of being evaluated one after the other by every lane.
+  // The kFused kernels inline the softplus here and the Box–Muller math in draw() (dhmc_math.h, the _inl twins): the one
+  // runs on the serial path between a leaf's reduction and the next leapfrog, the other at the head of every transition.
   __device__ __forceinline__ void logaddexp2(double a0, double b0, double a1, double b1,
                                              double* r0, double* r1) const {
     const bool odd = (lane & 1) != 0;
-    const double r = dm_logaddexp(odd ? a1 : a0, odd ? b1 : b0);
+    const double a = odd ? a1 : a0, b = odd ? b1 : b0;
+    double r;
+    if constexpr (kFused) r = dm_logaddexp_inl(a, b);
+    else r = dm_logaddexp(a, b);
     *r0 = __shfl_sync(0xffffffffu, r, 0);
     *r1 = __shfl_sync(0xffffffffu, r, 1);
   }
@@ -814,7 +819,7 @@ struct DeviceBackend {
   __device__ __forceinline__ double randexp(dm_rng_key key, uint32_t t, uint32_t j) {
     const uint32_t base = j & ~31u;
     if (base != rexp_base || t != rexp_t) {
-      rexp_cache = dm_randexp(key, t, base + (uint32_t)lane);
+      rexp_cache = dm_randexp(key, t, base + (uint32_t)lane);   // out of line: once per 32 draws, and inlined it spills more
       rexp_base = base; rexp_t = t;
     }
     return __shfl_sync(0xffffffffu, rexp_cache, (int)(j & 31u));
@@ -968,12 +973,17 @@ struct DeviceBackend {
       // lanes (T is even).  The even lane evaluates the pairs of even register slots, the
       // odd lane those of odd slots, and the halves are exchanged by one shuffle.
       const int odd = lane & 1;
+      uint32_t jp[EPL / 2];                       // the pair of register slots e, e + 1 that this lane evaluates
+#pragma unroll
+      for (int e = 0; e < EPL; e += 2) jp[e / 2] = (uint32_t)(((tid & ~1) + (e + odd) * T) >> 1);
+      // the kFused kernels evaluate the EPL / 2 pairs of this lane stage by stage, so that their chains overlap
+      double zp0[EPL / 2], zp1[EPL / 2];
+      if constexpr (kFused) dm_normal_pairs_inl(key, stream, t, jp, EPL / 2, zp0, zp1);
 #pragma unroll
       for (int e = 0; e < EPL; e += 2) {
-        const int my_e = e + odd;
-        const uint32_t j = (uint32_t)(((tid & ~1) + my_e * T) >> 1);
         double z0, z1;
-        dm_normal_pair(key, stream, t, j, &z0, &z1);
+        if constexpr (kFused) { z0 = zp0[e / 2]; z1 = zp1[e / 2]; }
+        else dm_normal_pair(key, stream, t, jp[e / 2], &z0, &z1);
         const double recv = __shfl_xor_sync(0xffffffffu, odd ? z0 : z1, 1);
         const double ze = odd ? recv : z0;        // element tid + e*T
         const double zo = odd ? z1 : recv;        // element tid + (e+1)*T

@@ -32,7 +32,11 @@
 #else
 #define DHMC_HD static inline
 #endif
-/* heavy transcendental bodies: optionally out of line on the device (code size) */
+/* heavy transcendental bodies: optionally out of line on the device (code size).  Each out-of-line function dm_f has a
+ * force-inlined twin dm_f_inl with the same body, for the call sites on a kernel's serial path (the tree's merges and
+ * the momentum draw of the diagonal-metric kernels, csrc/device_backend.cuh): there a call costs its latency, keeps
+ * independent evaluations from overlapping and pushes the values live across it to the stack.  Both twins perform the
+ * same operations, so they return the same bits. */
 #if defined(__CUDACC__) && defined(DHMC_NOINLINE_MATH)
 #define DHMC_HDH static __host__ __device__ __noinline__
 #else
@@ -151,7 +155,7 @@ DHMC_HDH double dm_exp(double x) {
 }
 
 /* ------------------------------------------------------------------- log */
-DHMC_HDH double dm_log(double x) {
+DHMC_HD double dm_log_inl(double x) {
   if (x != x) return x;
   if (x < 0.0) return dm_nan();
   if (x == 0.0) return -dm_inf();
@@ -192,6 +196,7 @@ DHMC_HDH double dm_log(double x) {
   double dk = (double)e;
   return dk * DM_LN2_HI + (f + (dk * DM_LN2_LO - s * (f - R)));
 }
+DHMC_HDH double dm_log(double x) { return dm_log_inl(x); }
 
 /* log1p via Kahan's correction; |error| a few ulp, deterministic. */
 DHMC_HD double dm_log1p(double x) {
@@ -264,9 +269,10 @@ static __constant__ double dm_d_logc[128] = DM_TAB_LOGC_INIT;
 #define DM_TI_DEFAULT(i) DM_TAB(invc, i)
 #define DM_TL_DEFAULT(i) DM_TAB(logc, i)
 /* softplus(-d) and exp(-d); tables from constant memory on the device (uniform indices: one access) */
-DHMC_HDH double dm_softplus_neg_exp(double d, double* t_out) {
+DHMC_HD double dm_softplus_neg_exp_inl(double d, double* t_out) {
   DM_SOFTPLUS_NEG_BODY(DM_TE_DEFAULT, DM_TI_DEFAULT, DM_TL_DEFAULT)
 }
+DHMC_HDH double dm_softplus_neg_exp(double d, double* t_out) { return dm_softplus_neg_exp_inl(d, t_out); }
 DHMC_HD double dm_softplus_neg(double d) {
   double t;
   return dm_softplus_neg_exp(d, &t);
@@ -287,12 +293,15 @@ DHMC_HD double dm_tabs_entry(int i) {
 
 /* log(exp(a)+exp(b)), LogExpFunctions.logaddexp semantics
  * (call sites src/trees.jl:145, src/NUTS.jl:70): equal arguments (incl. both
- * -Inf) give a + log(2); otherwise max + log1pexp(-|a-b|). */
-DHMC_HD double dm_logaddexp(double a, double b) {
-  double d = (a == b) ? 0.0 : dm_fabs(a - b);
-  double mx = dm_max_nan(a, b);
-  return mx + dm_softplus_neg(d);
-}
+ * -Inf) give a + log(2); otherwise max + log1pexp(-|a-b|).  SFX selects the
+ * out-of-line softplus (empty) or its inlined twin (_inl). */
+#define DM_LOGADDEXP_BODY(SFX)                                                  \
+  double d = (a == b) ? 0.0 : dm_fabs(a - b);                                   \
+  double mx = dm_max_nan(a, b);                                                 \
+  double t;                                                                     \
+  return mx + dm_softplus_neg_exp##SFX(d, &t);
+DHMC_HD double dm_logaddexp(double a, double b) { DM_LOGADDEXP_BODY() }
+DHMC_HD double dm_logaddexp_inl(double a, double b) { DM_LOGADDEXP_BODY(_inl) }
 
 /* log(1+exp(x)) (logistic-regression likelihood) */
 DHMC_HD double dm_log1pexp(double x) {
@@ -305,7 +314,7 @@ DHMC_HD double dm_log1pexp(double x) {
 /* -------------------------------------------------- sin/cos of 2*pi*u */
 #define DM_PIO4 7.85398163397448309616e-01
 /* u in [0,1): returns cos(2 pi u), sin(2 pi u); octant reduction is exact. */
-DHMC_HDH void dm_sincos2pi(double u, double* sn, double* cs) {
+DHMC_HD void dm_sincos2pi_inl(double u, double* sn, double* cs) {
   double a = 8.0 * u;
   double jf = dm_floor(a);
   int j = ((int)jf) & 7;
@@ -348,6 +357,7 @@ DHMC_HDH void dm_sincos2pi(double u, double* sn, double* cs) {
   }
   *sn = ss; *cs = cc;
 }
+DHMC_HDH void dm_sincos2pi(double u, double* sn, double* cs) { dm_sincos2pi_inl(u, sn, cs); }
 
 /* ------------------------------------------------------- Philox-4x32-10 */
 typedef struct { uint32_t v[4]; } dm_u32x4;
@@ -360,8 +370,8 @@ DHMC_HD uint32_t dm_mulhi32(uint32_t a, uint32_t b) {
 #endif
 }
 
-DHMC_HDH dm_u32x4 dm_philox4x32_10(uint32_t c0, uint32_t c1, uint32_t c2,
-                                   uint32_t c3, uint32_t k0, uint32_t k1) {
+DHMC_HD dm_u32x4 dm_philox4x32_10_inl(uint32_t c0, uint32_t c1, uint32_t c2,
+                                      uint32_t c3, uint32_t k0, uint32_t k1) {
   const uint32_t M0 = 0xD2511F53u, M1 = 0xCD9E8D57u;
   const uint32_t W0 = 0x9E3779B9u, W1 = 0xBB67AE85u;
 #if defined(__CUDA_ARCH__)
@@ -378,6 +388,10 @@ DHMC_HDH dm_u32x4 dm_philox4x32_10(uint32_t c0, uint32_t c1, uint32_t c2,
   dm_u32x4 o;
   o.v[0] = c0; o.v[1] = c1; o.v[2] = c2; o.v[3] = c3;
   return o;
+}
+DHMC_HDH dm_u32x4 dm_philox4x32_10(uint32_t c0, uint32_t c1, uint32_t c2,
+                                   uint32_t c3, uint32_t k0, uint32_t k1) {
+  return dm_philox4x32_10_inl(c0, c1, c2, c3, k0, k1);
 }
 
 /* RNG streams: one Philox block = (idx, transition, chain_lo, stream|chain_hi) */
@@ -402,11 +416,13 @@ DHMC_HD dm_rng_key dm_make_key(uint64_t seed, uint64_t chain) {
   k.chain_hi24 = (uint32_t)((chain >> 32) & 0xFFFFFFu);
   return k;
 }
+/* The composites below come in the same two forms: SFX empty calls the out-of-line bodies, SFX = _inl their twins. */
+#define DM_RNG_BLOCK_BODY(SFX)                                                  \
+  return dm_philox4x32_10##SFX(idx, t, k.chain_lo, (stream << 24) | k.chain_hi24, k.k0, k.k1);
 DHMC_HD dm_u32x4 dm_rng_block(dm_rng_key k, uint32_t stream, uint32_t t,
-                               uint32_t idx) {
-  return dm_philox4x32_10(idx, t, k.chain_lo, (stream << 24) | k.chain_hi24,
-                          k.k0, k.k1);
-}
+                               uint32_t idx) { DM_RNG_BLOCK_BODY() }
+DHMC_HD dm_u32x4 dm_rng_block_inl(dm_rng_key k, uint32_t stream, uint32_t t,
+                                   uint32_t idx) { DM_RNG_BLOCK_BODY(_inl) }
 /* 52-bit uniform strictly inside (0,1): (n + 1/2) * 2^-52, exact */
 DHMC_HD double dm_u01(uint32_t a, uint32_t b) {
   uint64_t n = ((uint64_t)a << 20) | (uint64_t)(b >> 12);
@@ -422,6 +438,33 @@ DHMC_HD void dm_normal_pair(dm_rng_key k, uint32_t stream, uint32_t t,
   double sn, cs;
   dm_sincos2pi(u2, &sn, &cs);
   *z0 = rad * cs; *z1 = rad * sn;
+}
+/* n independent pairs at once, z0[h], z1[h] for pair j[h]: each pair takes exactly the operations of dm_normal_pair (inlined
+ * bodies), but the Philox blocks, the logs and the sin/cos of all pairs are evaluated stage by stage, so that the n
+ * dependency chains can overlap instead of running one after the other. */
+DHMC_HD void dm_normal_pairs_inl(dm_rng_key k, uint32_t stream, uint32_t t, const uint32_t* j, int n,
+                                 double* z0, double* z1) {
+#if defined(__CUDA_ARCH__)
+#pragma unroll
+#endif
+  for (int h = 0; h < n; ++h) {
+    dm_u32x4 r = dm_rng_block_inl(k, stream, t, j[h]);
+    z0[h] = dm_u01(r.v[0], r.v[1]);                                          /* u1 */
+    z1[h] = dm_u01(r.v[2], r.v[3]);                                          /* u2 */
+  }
+#if defined(__CUDA_ARCH__)
+#pragma unroll
+#endif
+  for (int h = 0; h < n; ++h) z0[h] = dm_sqrt(-2.0 * dm_log_inl(z0[h]));     /* rad */
+#if defined(__CUDA_ARCH__)
+#pragma unroll
+#endif
+  for (int h = 0; h < n; ++h) {
+    double sn, cs;
+    dm_sincos2pi_inl(z1[h], &sn, &cs);
+    const double rad = z0[h];
+    z0[h] = rad * cs; z1[h] = rad * sn;
+  }
 }
 DHMC_HD double dm_normal_elem(dm_rng_key k, uint32_t stream, uint32_t t,
                               uint32_t i) {
