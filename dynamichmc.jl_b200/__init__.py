@@ -8,4 +8,4 @@ from .api import (ArgumentError, DiagNormal, Diagonal, DualAveraging, DynamicHMC
                   MCMCSteps, ProblemBatch, RaggedProblemBatch, Results, StandardNormal, Symmetric, SymmetricPooled, TuningNUTS, UserLogDensity, compile_user_model,
                   default_warmup_stages,
                   fixed_stepsize_warmup_stages, mcmc_keep_warmup, mcmc_next_step, mcmc_steps, mcmc_with_warmup,
-                  pool_posterior_matrices, results_by_problem, stack_posterior_matrices)
+                  pool_posterior_matrices, results_by_problem, stack_posterior_matrices, summarize_with_warmup)

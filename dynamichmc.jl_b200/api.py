@@ -689,6 +689,51 @@ class Engine:
                                              L.ptr(stats), L.ptr(ld)))
         return dict(posterior_matrix=post, tree_statistics=stats, logdensities=ld)
 
+    def mcmc_summary(self, N, thin=1, reference=None, stats=False):
+        """N transitions as mcmc (same draws, same final state and transition count), every thin-th kept and folded on the
+        device into per-(problem, parameter) statistics instead of being returned (dhmc_mcmc_summary, DESIGN §4.4).
+        `reference` [P, D] adds the SBC rank of each reference value among its problem's kept draws.  Returns a dict of
+        [P, D] arrays — mean, sd, mcse, ess (between-chain batch means, not the Geyer ESS), rhat (split-R̂), rank (−1
+        without a reference), draws — plus `record` [P, D, SUMMARY_FIELDS], the mergeable form (diagnostics.merge_summaries,
+        dhmc_summary_merge), and with stats=True the kept transitions' tree_statistics and logdensities [K, N // thin].
+        A chain that fails is left out of its problem's statistics; the call raises as mcmc does, and the exception's
+        debug_information["summary"] holds the summary of the other chains."""
+        _argcheck(N >= 1 and thin >= 1 and N % thin == 0, "N ≥ 1, thin ≥ 1 and N a multiple of thin")
+        _argcheck(N // thin >= 4, "at least 4 kept draws per chain (N / thin ≥ 4)")
+        P = self.ℓ.n_problems if isinstance(self.ℓ, ProblemBatch) else 1
+        ref = None
+        if reference is not None:
+            ref = np.ascontiguousarray(reference, float)
+            _argcheck(ref.shape == (P, self.D), f"reference: [P, D] = ({P}, {self.D})")
+        record = np.zeros((P, self.D, L.SUMMARY_FIELDS))
+        n = N // thin
+        st = np.zeros((self.K, n), dtype=L.tree_stats_dtype) if stats else None
+        ld = np.empty((self.K, n)) if stats else None
+        rc = self._lib.dhmc_mcmc_summary(self._h, N, thin, L.ptr(ref), L.ptr(record), L.ptr(st), L.ptr(ld))
+        if rc not in (L.DHMC_OK, L.DHMC_ENUMERIC):
+            self._ck(rc)
+        out = self.summary_finish(record)
+        out["record"] = record
+        if stats:
+            out.update(tree_statistics=st, logdensities=ld)
+        try:
+            self._ck(rc)
+        except (ArgumentError, DynamicHMCError) as e:
+            e.debug_information["summary"] = out
+            raise
+        return out
+
+    def summary_finish(self, record):
+        """dhmc_summary_finish of a record [P, D, SUMMARY_FIELDS] → mean, sd, mcse, ess, rhat, rank, draws [P, D]."""
+        rec = np.ascontiguousarray(record, float)
+        P, D = rec.shape[:2]
+        _argcheck(rec.shape == (P, D, L.SUMMARY_FIELDS), "record: [P, D, SUMMARY_FIELDS]")
+        out = {k: np.empty((P, D)) for k in ("mean", "sd", "mcse", "ess", "rhat")}
+        out.update(rank=np.empty((P, D), np.int64), draws=np.empty((P, D), np.int64))
+        self._ck(self._lib.dhmc_summary_finish(L.ptr(rec), D, P, *(L.ptr(out[k]) for k in
+                                                                      ("mean", "sd", "mcse", "ess", "rhat", "rank", "draws"))))
+        return out
+
     def host_alloc(self, shape, dtype=np.float64):
         """Page-locked, device-mapped numpy array on the NUMA node of this engine's GPU (dhmc_host_alloc).
         Freed with the engine (or host_free)."""
@@ -875,11 +920,9 @@ def _default_chains(ℓ, chains, chain_offset):
     return ℓ.chains - chain_offset if isinstance(ℓ, ProblemBatch) else 1
 
 
-def mcmc_keep_warmup(seed, ℓ, N, chains=None, initialization=None, warmup_stages=None,
-                     algorithm=None, keep_warmup=True, device=0, chain_offset=0, engine_opts=None, reporter=None):
-    """src/mcmc.jl:521-532 for `chains` chains at once (default 1; for a ProblemBatch every chain of the batch from
-    chain_offset on)."""
-    chains = _default_chains(ℓ, chains, chain_offset)
+def _warm_up(seed, ℓ, chains, initialization, warmup_stages, algorithm, keep_warmup, device, chain_offset, engine_opts,
+             reporter):
+    """the warm-up half of mcmc_keep_warmup: a new Engine taken through every stage → (engine, per-stage results)"""
     stages = default_warmup_stages() if warmup_stages is None else warmup_stages
     eng = Engine(ℓ, chains, seed=seed, algorithm=algorithm, device=device, chain_offset=chain_offset,
                  **(engine_opts or {}))
@@ -897,6 +940,16 @@ def mcmc_keep_warmup(seed, ℓ, N, chains=None, initialization=None, warmup_stag
             raise ArgumentError(f"unknown warmup stage {stage!r}")
         _report(reporter, "warmup stage finished", stage=i + 1, of=len(stages), kind=type(stage).__name__,
                 transitions=getattr(stage, "N", 0), chains=chains)
+    return eng, warm
+
+
+def mcmc_keep_warmup(seed, ℓ, N, chains=None, initialization=None, warmup_stages=None,
+                     algorithm=None, keep_warmup=True, device=0, chain_offset=0, engine_opts=None, reporter=None):
+    """src/mcmc.jl:521-532 for `chains` chains at once (default 1; for a ProblemBatch every chain of the batch from
+    chain_offset on)."""
+    chains = _default_chains(ℓ, chains, chain_offset)
+    eng, warm = _warm_up(seed, ℓ, chains, initialization, warmup_stages, algorithm, keep_warmup, device, chain_offset,
+                         engine_opts, reporter)
     inf = eng.mcmc(N)
     _report(reporter, "inference finished", transitions=N, chains=chains)
     st = eng.get_state(("minv", "eps"))
@@ -914,6 +967,23 @@ def mcmc_with_warmup(seed, ℓ, N, chains=None, initialization=None, warmup_stag
                          device=device, chain_offset=chain_offset, engine_opts=engine_opts, reporter=reporter)
     r["engine"].close()
     return r["inference"]
+
+
+def summarize_with_warmup(seed, ℓ, N, thin=1, reference=None, chains=None, initialization=None, warmup_stages=None,
+                          algorithm=None, device=0, chain_offset=0, engine_opts=None, reporter=None):
+    """mcmc_with_warmup ending in Engine.mcmc_summary instead of Results: the warm-up, then N transitions whose every
+    thin-th draw is folded on the device into per-(problem, parameter) mean, sd, mcse, ess, rhat and — with a reference
+    [P, D] — SBC ranks.  Memory and traffic do not grow with N: simulation-based calibration over a ProblemBatch of
+    thousands of data sets is one call.  Returns the dict of Engine.mcmc_summary."""
+    chains = _default_chains(ℓ, chains, chain_offset)
+    eng, _ = _warm_up(seed, ℓ, chains, initialization, warmup_stages, algorithm, False, device, chain_offset,
+                      engine_opts, reporter)
+    try:
+        out = eng.mcmc_summary(N, thin=thin, reference=reference)
+        _report(reporter, "inference finished", transitions=N, chains=chains)
+    finally:
+        eng.close()
+    return out
 
 
 class MCMCSteps:

@@ -358,6 +358,10 @@ struct dhmc_handle {
   ncclComm_t comm = nullptr;        // multi-GPU: one communicator per handle (dhmc_comm_init)
   int comm_nranks = 1, comm_rank = 0;
   double last_comm_ms = 0;
+  // streaming summary (dhmc_mcmc_summary): grow-only device arena of the SummaryArgs arrays, and the struct itself
+  void* sum_buf = nullptr;
+  size_t sum_bytes = 0;
+  SummaryArgs* sum_args = nullptr;
   std::string err;
 };
 
@@ -592,6 +596,7 @@ int dhmc_destroy(dhmc_handle* h) {
   cudaFree(h->minv_dense); cudaFree(h->wt); cudaFree(h->covt); cudaFree(h->dense_tmp); cudaFree(h->minv_pad); cudaFree(h->mean_pool);
   cudaFree(h->lX); cudaFree(h->lXt); cudaFree(h->ly); cudaFree(h->lr); cudaFree(h->lXp); cudaFree(h->problems);
   cudaFree(h->tmp_b); cudaFree(h->tmp_bd); cudaFree(h->tmp_dir);
+  cudaFree(h->sum_buf); cudaFree(h->sum_args);
   for (void* r : h->registered) cudaHostUnregister(r);
   if (h->comm) dhmc_comm_destroy(h);
   if (h->ev0) cudaEventDestroy(h->ev0);
@@ -1109,7 +1114,8 @@ static bool host_mapped(const void* p, void** dev) {
 static int run_nuts(dhmc_handle* h, int N, const AdaptConfig& cfg, double lambda, const double* p_over_host,
                     const uint32_t* dir_over_host, double* posterior, dhmc_tree_stats* stats,
                     double* eps_used, double* logdens, bool outputs_on_device, bool advance_t,
-                    const double* q_host = nullptr, int thin = 1, bool pool_metric = false) {
+                    const double* q_host = nullptr, int thin = 1, bool pool_metric = false,
+                    const SummaryArgs* summary = nullptr) {
   if ((!h->has_position && !q_host) || !h->has_eps) { h->err = "set position and step size (or run the initial search) first"; return DHMC_EARG; }
   const auto tr0 = std::chrono::steady_clock::now();
   auto tr_ms = [&] { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - tr0).count(); };
@@ -1178,6 +1184,7 @@ static int run_nuts(dhmc_handle* h, int N, const AdaptConfig& cfg, double lambda
   a.out_lq = (double*)out[3].dev;
   if (cfg.metric == DHMC_METRIC_SYMMETRIC) a.covt = h->covt;
   if (pool_metric) a.mean_out = h->mean_pool;
+  a.summary = summary;
   const size_t out_bytes = posterior ? sizeof(double) * B * n * D : 0;
   // chunks must stay many waves long, or the ragged tail of every chunk idles the SMs
   // chunks overlap the staged downloads (and the upload of q_host) with the sampling of the next chunk; with direct
@@ -1372,6 +1379,146 @@ int dhmc_mcmc_dev(dhmc_handle* h, int32_t N, double* posterior, dhmc_tree_stats*
   if (N == 0) return DHMC_OK;
   AdaptConfig cfg{};
   return run_nuts(h, N, cfg, 0.0, nullptr, nullptr, posterior, stats, nullptr, logdens, true, true);
+}
+
+// ------------------------------------------------------------------ streaming posterior summary (DESIGN §4.4)
+// record [DHMC_SUMMARY_FIELDS, D, P] column-major: the fields of (parameter d, problem p) at (p·D + d)·F
+static double* summary_cell(double* record, int64_t D, int64_t p, int64_t d) { return record + ((size_t)p * D + d) * DHMC_SUMMARY_FIELDS; }
+
+int dhmc_mcmc_summary(dhmc_handle* h, int32_t N, int32_t thin, const double* reference, double* record, dhmc_tree_stats* stats,
+                      double* logdens) {
+  if (!h) return DHMC_EARG;
+  if (N < 1 || thin < 1 || N % thin != 0) { h->err = "dhmc_mcmc_summary: N ≥ 1, thin ≥ 1 and N a multiple of thin"; return DHMC_EARG; }
+  const int n_keep = N / thin;
+  if (n_keep < 4) { h->err = "dhmc_mcmc_summary: at least 4 kept draws per chain (N / thin ≥ 4)"; return DHMC_EARG; }
+  if (!record) { h->err = "dhmc_mcmc_summary: record is NULL"; return DHMC_EARG; }
+  if (!h->has_position || !h->has_eps) { h->err = "set position and step size (or run the initial search) first"; return DHMC_EARG; }
+  CK(cudaSetDevice(h->cfg.device));
+  const size_t D = (size_t)h->cfg.dim, B = (size_t)h->cfg.n_chains;
+  const int64_t K = h->batch_k, off = h->cfg.chain_offset;
+  const size_t P = K ? (size_t)h->batch_p : 1, PD = P * D, rows = (size_t)h->grid * h->G * 3 * D;
+  // one grow-only arena, 8-byte elements throughout: acc [P][5][D], shift [P][D], ref [P][D], row [grid·G][3][D],
+  // below [P][D], chains [P]
+  const size_t need = sizeof(double) * (8 * PD + rows + P);
+  if (need > h->sum_bytes) {
+    cudaFree(h->sum_buf); h->sum_buf = nullptr; h->sum_bytes = 0;
+    CK(cudaMalloc(&h->sum_buf, need));
+    h->sum_bytes = need;
+  }
+  if (!h->sum_args) CK(cudaMalloc(&h->sum_args, sizeof(SummaryArgs)));
+  double* acc = (double*)h->sum_buf;
+  double* shift = acc + 5 * PD;
+  double* ref = shift + PD;
+  double* row = ref + PD;
+  unsigned long long* below = (unsigned long long*)(row + rows);
+  unsigned long long* chains = below + PD;
+  CK(cudaMemsetAsync(acc, 0, sizeof(double) * 5 * PD, h->stream));
+  CK(cudaMemsetAsync(below, 0, sizeof(unsigned long long) * (PD + P), h->stream));
+  if (reference) CK(cudaMemcpyAsync(ref, reference, sizeof(double) * PD, cudaMemcpyHostToDevice, h->stream));
+  // shift of problem p: the position of its first local chain, max(p·K − off, 0); problems p0 … p1 have local chains.  Past
+  // the first, those chains are K apart: one strided copy (a first problem entered in its middle takes one more).
+  const int64_t p0 = K ? off / K : 0, p1 = K ? (off + (int64_t)B - 1) / K : 0;
+  const int64_t pa = (K && off % K) ? p0 + 1 : p0;
+  if (pa > p0) CK(cudaMemcpyAsync(shift + p0 * D, h->q, sizeof(double) * D, cudaMemcpyDeviceToDevice, h->stream));
+  if (p1 >= pa)
+    CK(cudaMemcpy2DAsync(shift + pa * D, sizeof(double) * D, h->q + (size_t)(K ? pa * K - off : 0) * D, sizeof(double) * D * (size_t)(K ? K : 1),
+                         sizeof(double) * D, (size_t)(p1 - pa + 1), cudaMemcpyDeviceToDevice, h->stream));
+  const SummaryArgs sa{row, shift, reference ? ref : nullptr, acc, below, chains, n_keep / 2};
+  CK(cudaMemcpyAsync(h->sum_args, &sa, sizeof sa, cudaMemcpyHostToDevice, h->stream));
+  AdaptConfig cfg{};
+  const int rc = run_nuts(h, N, cfg, 0.0, nullptr, nullptr, nullptr, stats, nullptr, logdens, false, true, nullptr, thin, false,
+                          h->sum_args);
+  if (rc != DHMC_OK && rc != DHMC_ENUMERIC) return rc;    // a chain that failed is left out of its problem's sums
+  std::vector<double> hacc(5 * PD), hshift(PD);
+  std::vector<unsigned long long> hcnt(PD + P);
+  CK(cudaMemcpyAsync(hacc.data(), acc, sizeof(double) * hacc.size(), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaMemcpyAsync(hshift.data(), shift, sizeof(double) * PD, cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaMemcpyAsync(hcnt.data(), below, sizeof(unsigned long long) * hcnt.size(), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  for (size_t p = 0; p < P; ++p) {
+    const double M = (double)hcnt[PD + p], m = 2.0 * M;
+    const double* a = &hacc[p * 5 * D];
+    for (size_t d = 0; d < D; ++d) {
+      double* r = summary_cell(record, (int64_t)D, (int64_t)p, (int64_t)d);
+      r[DHMC_SUMMARY_CHAINS] = M;
+      r[DHMC_SUMMARY_NKEEP] = (double)n_keep;
+      r[DHMC_SUMMARY_BELOW] = reference ? (double)hcnt[p * D + d] : dm_nan();
+      if (M == 0) {
+        r[DHMC_SUMMARY_MEAN] = r[DHMC_SUMMARY_SS_SEQ] = r[DHMC_SUMMARY_M2] = r[DHMC_SUMMARY_SS_CHAIN] = 0.0;
+        continue;
+      }
+      const double s1 = a[d], s2 = a[D + d], c1 = a[3 * D + d], c2 = a[4 * D + d];
+      r[DHMC_SUMMARY_MEAN] = hshift[p * D + d] + s1 / m;
+      r[DHMC_SUMMARY_SS_SEQ] = std::max(0.0, s2 - s1 * s1 / m);
+      r[DHMC_SUMMARY_M2] = a[2 * D + d];
+      r[DHMC_SUMMARY_SS_CHAIN] = std::max(0.0, c2 - c1 * c1 / M);
+    }
+  }
+  return rc;
+}
+
+int dhmc_summary_merge(double* record, const double* other, int64_t D, int64_t P) {
+  if (!record || !other || D < 1 || P < 1) return DHMC_EARG;
+  const size_t n = (size_t)D * (size_t)P;
+  for (size_t i = 0; i < n; ++i) {      // every count must agree before anything is written
+    const double* a = record + i * DHMC_SUMMARY_FIELDS;
+    const double* b = other + i * DHMC_SUMMARY_FIELDS;
+    if (a[DHMC_SUMMARY_CHAINS] > 0 && b[DHMC_SUMMARY_CHAINS] > 0 && a[DHMC_SUMMARY_NKEEP] != b[DHMC_SUMMARY_NKEEP]) return DHMC_EARG;
+  }
+  for (size_t i = 0; i < n; ++i) {
+    double* a = record + i * DHMC_SUMMARY_FIELDS;
+    const double* b = other + i * DHMC_SUMMARY_FIELDS;
+    const double ma = a[DHMC_SUMMARY_CHAINS], mb = b[DHMC_SUMMARY_CHAINS], below = a[DHMC_SUMMARY_BELOW] + b[DHMC_SUMMARY_BELOW];
+    if (mb == 0) { a[DHMC_SUMMARY_BELOW] = below; continue; }
+    if (ma == 0) {
+      for (int f = 0; f < DHMC_SUMMARY_FIELDS; ++f) a[f] = b[f];
+      a[DHMC_SUMMARY_BELOW] = below;
+      continue;
+    }
+    // Chan, Golub and LeVeque: pooled mean and centred sums of squares of two groups (2 sequences per chain)
+    const double M = ma + mb, delta = b[DHMC_SUMMARY_MEAN] - a[DHMC_SUMMARY_MEAN];
+    a[DHMC_SUMMARY_MEAN] = a[DHMC_SUMMARY_MEAN] + delta * (mb / M);
+    a[DHMC_SUMMARY_SS_SEQ] = a[DHMC_SUMMARY_SS_SEQ] + b[DHMC_SUMMARY_SS_SEQ] + delta * delta * (2.0 * ma * mb / M);
+    a[DHMC_SUMMARY_M2] = a[DHMC_SUMMARY_M2] + b[DHMC_SUMMARY_M2];
+    a[DHMC_SUMMARY_SS_CHAIN] = a[DHMC_SUMMARY_SS_CHAIN] + b[DHMC_SUMMARY_SS_CHAIN] + delta * delta * (ma * mb / M);
+    a[DHMC_SUMMARY_CHAINS] = M;
+    a[DHMC_SUMMARY_BELOW] = below;
+  }
+  return DHMC_OK;
+}
+
+int dhmc_summary_finish(const double* record, int64_t D, int64_t P, double* mean, double* sd, double* mcse, double* ess,
+                        double* rhat, int64_t* rank, int64_t* draws) {
+  if (!record || D < 1 || P < 1) return DHMC_EARG;
+  const size_t n_cells = (size_t)D * (size_t)P;
+  for (size_t i = 0; i < n_cells; ++i) {
+    const double* r = record + i * DHMC_SUMMARY_FIELDS;
+    const double M = r[DHMC_SUMMARY_CHAINS], m = 2.0 * M, n = std::floor(r[DHMC_SUMMARY_NKEEP] / 2.0);
+    const double below = r[DHMC_SUMMARY_BELOW];
+    if (rank) rank[i] = below == below ? (int64_t)below : -1;
+    if (draws) draws[i] = (int64_t)(r[DHMC_SUMMARY_NKEEP] * M);
+    double o_mean = dm_nan(), o_sd = dm_nan(), o_mcse = dm_nan(), o_ess = dm_nan(), o_rhat = dm_nan();
+    if (M > 0) {
+      const double ss = r[DHMC_SUMMARY_SS_SEQ], m2 = r[DHMC_SUMMARY_M2];
+      const double var = (m2 + n * ss) / (m * n - 1.0);               // pooled variance of the 2n·M draws
+      const double W = m2 / (m * (n - 1.0));                          // mean within-sequence variance
+      const double var_plus = (n - 1.0) / n * W + ss / (m - 1.0);     // (n−1)/n·W + var(μ_s), as ess_rhat_groups
+      o_mean = r[DHMC_SUMMARY_MEAN];
+      o_sd = std::sqrt(var);
+      o_rhat = std::sqrt(var_plus / W);
+      if (M >= 2) {
+        const double var_c = r[DHMC_SUMMARY_SS_CHAIN] / (M - 1.0) / M;   // squared standard error of the chain means' mean
+        o_mcse = std::sqrt(var_c);
+        if (var_plus > 0.0) o_ess = var / var_c;
+      }
+    }
+    if (mean) mean[i] = o_mean;
+    if (sd) sd[i] = o_sd;
+    if (mcse) mcse[i] = o_mcse;
+    if (ess) ess[i] = o_ess;
+    if (rhat) rhat[i] = o_rhat;
+  }
+  return DHMC_OK;
 }
 
 int dhmc_tree_summary_dev(dhmc_handle* h, const dhmc_tree_stats* stats_dev, int32_t N, int64_t* depth_counts,

@@ -31,6 +31,24 @@ struct ProblemDesc {
   int N, ld;
 };
 
+// Streaming posterior summary (dhmc_mcmc_summary, DESIGN §4.4): the kept draws of every chain are folded into Welford
+// moments (the metric window's two reserved slots) and, at chain end, into per-problem sums; no draw is written out.
+//   row    [grid·G][3][D]  per chain group: sequence 0's mean and M2, and the count of kept draws below the reference
+//   shift  [P][D]          the position of the problem's first local chain at call start (keeps the sums free of cancellation)
+//   ref    [P][D] or null  the reference of the rank statistic
+//   acc    [P][5][D]       Σ(μ_s − s), Σ(μ_s − s)², Σ M2_s over sequences; Σ(μ_c − s), Σ(μ_c − s)² over chains
+//   below  [P][D]          Σ #{kept draws with θ < reference} (exact)
+//   chains [P]             chains that completed the call
+struct SummaryArgs {
+  double* row;
+  const double* shift;
+  const double* ref;
+  double* acc;
+  unsigned long long* below;
+  unsigned long long* chains;
+  int n;                        // draws per sequence: ⌊N_keep / 2⌋
+};
+
 struct KArgs {
   int D, B, T, W;
   unsigned long long seed;
@@ -79,6 +97,7 @@ struct KArgs {
   int batch_k;
   const ProblemDesc* problems;
   int red_groups;               // groups of the reduction buffer (smem_layout rg) of the kernels with DeviceBackend::kFused
+  const SummaryArgs* summary;   // k_nuts: fold the kept draws into a streaming summary (device struct; null: off)
 #if defined(DHMC_PHASE_CLOCKS)
   unsigned long long* phase_clocks;   // leaf profile: kPhCount counters per CTA (nuts_machine.cuh)
 #endif
@@ -228,6 +247,14 @@ __device__ __forceinline__ void store_vec(const DeviceBackend<EPL, FAM, W, DN, G
 }
 
 // ------------------------------------------------------------------ k_nuts
+// problem of local chain c (as load_chain)
+__device__ __forceinline__ size_t summary_problem(const KArgs& a, long c) {
+  return a.batch_k ? (size_t)((unsigned)(a.chain_offset + c) / (unsigned)a.batch_k) : 0;
+}
+template <class Bk>
+__device__ __noinline__ void summary_draw(const SummaryArgs* sp, double** slot_tab, int n_slots, int s_zq, int tid, int grp, int D,
+                                         size_t p, int j);
+
 template <int EPL, int FAM, int W, bool DN, int G, bool DP>
 struct DrawSink {
   DeviceBackend<EPL, FAM, W, DN, G, DP>& b;
@@ -251,8 +278,90 @@ struct DrawSink {
       if (a.out_lq) a.out_lq[row] = b.lq;
       if (a.out_eps) a.out_eps[row] = e;
     }
+    if (a.summary)
+      summary_draw<DeviceBackend<EPL, FAM, W, DN, G, DP>>(a.summary, b.slot_tab, b.n_slots, b.top().s_zq, b.tid, b.grp, a.D,
+                                                          summary_problem(a, c), n);
   }
 };
+
+// ---- streaming summary (DESIGN §4.4), out of line and reached only when KArgs::summary is set, so that its body costs the
+// sampling path no registers (ptxas still saves a few bytes around the two calls: benchmarks/streaming_summary_ptxas.md).
+// The functions get the chain's slot table, not its backend (whose registers would have to move to memory to be passed); the kept position is read from the slot the transition loaded it from (the proposal ζ),
+// and the Welford update is the metric window's own (metric_reset / metric_push on the two reserved slots), run on a view
+// that holds only what those read.  Every thread touches its own elements i = tid + e·T, so nothing here synchronises.
+template <class Bk>
+__device__ __forceinline__ Bk welford_view(double** slot_tab, int n_slots, int tid, int D) {
+  Bk w;
+  w.slot_tab = slot_tab; w.n_slots = n_slots; w.tid = tid; w.D = D;
+  return w;
+}
+template <class Bk>
+__device__ __forceinline__ double* summary_row(const SummaryArgs& s, int grp, int D) {
+  const size_t group = Bk::G > 1 ? (size_t)blockIdx.x * Bk::G + grp : (size_t)blockIdx.x;
+  return s.row + group * 3 * (size_t)D;
+}
+// kept draw j: sequence 0 is draws [0, n), sequence 1 draws [n, 2n); an odd last draw counts for the rank only
+template <class Bk>
+__device__ __noinline__ void summary_draw(const SummaryArgs* sp, double** slot_tab, int n_slots, int s_zq, int tid, int grp, int D,
+                                         size_t p, int j) {
+  constexpr int EPL = sizeof(Bk::q) / sizeof(double), T = Bk::T;
+  const SummaryArgs& s = *sp;
+  Bk w = welford_view<Bk>(slot_tab, n_slots, tid, D);
+  double* row = summary_row<Bk>(s, grp, D);
+  const int n = s.n;
+  w.ld_q(s_zq);
+  if (j < 2 * n) {
+    const int k = j < n ? j + 1 : j - n + 1;          // place in its sequence (1-based)
+    if (k == 1) w.metric_reset(DHMC_METRIC_DIAGONAL);
+    w.metric_push(DHMC_METRIC_DIAGONAL, k);
+    if (j == n - 1) {                                 // sequence 0 is complete: park its mean and M2, free the slots
+      const double* m = w.slot(n_slots - 1);
+      const double* sv = w.slot(n_slots - 2);
+#pragma unroll
+      for (int e = 0; e < EPL; ++e) {
+        const int i = tid + e * T;
+        if (i < D) { row[i] = m[e * T]; row[D + i] = sv[e * T]; }
+      }
+    }
+  }
+  if (s.ref) {
+    const double* ref = s.ref + p * D;
+#pragma unroll
+    for (int e = 0; e < EPL; ++e) {
+      const int i = tid + e * T;
+      if (i < D) {
+        const double below = w.q[e] < ref[i] ? 1.0 : 0.0;
+        row[2 * D + i] = j == 0 ? below : row[2 * D + i] + below;
+      }
+    }
+  }
+}
+// chain end (the chain completed the call): fold its two sequences into its problem's sums
+template <class Bk>
+__device__ __noinline__ void summary_fold(const SummaryArgs* sp, double** slot_tab, int n_slots, int tid, int grp, int Di, size_t p) {
+  constexpr int EPL = sizeof(Bk::q) / sizeof(double), T = Bk::T;
+  const SummaryArgs& s = *sp;
+  const double* row = summary_row<Bk>(s, grp, Di);
+  const double* m = slot_tab[n_slots - 1] + tid;
+  const double* sv = slot_tab[n_slots - 2] + tid;
+  const size_t D = (size_t)Di;
+  double* acc = s.acc + p * 5 * D;
+#pragma unroll
+  for (int e = 0; e < EPL; ++e) {
+    const int i = tid + e * T;
+    if (i < Di) {
+      const double sh = s.shift[p * D + i];
+      const double d0 = row[i] - sh, d1 = m[e * T] - sh, dc = 0.5 * (d0 + d1);   // μ_c: the mean of both sequences
+      atomicAdd(acc + i, d0 + d1);
+      atomicAdd(acc + D + i, d0 * d0 + d1 * d1);
+      atomicAdd(acc + 2 * D + i, row[D + i] + sv[e * T]);
+      atomicAdd(acc + 3 * D + i, dc);
+      atomicAdd(acc + 4 * D + i, dc * dc);
+      if (s.ref) atomicAdd(s.below + p * D + i, (unsigned long long)row[2 * D + i]);
+    }
+  }
+  if (tid == 0) atomicAdd(s.chains + p, 1ull);
+}
 
 template <int EPL, int FAM, int W, bool DN, int G = 1, bool DP = false>
 __global__ void __launch_bounds__(32 * W * G, G > 1 ? 1 : min_ctas(W, EPL)) k_nuts(const KArgs a) {
@@ -291,6 +400,8 @@ __global__ void __launch_bounds__(32 * W * G, G > 1 ? 1 : min_ctas(W, EPL)) k_nu
       if (m.status) atomicOr(a.status + c, m.status);
       atomicAdd(a.total_steps, (unsigned long long)m.steps_out);
     }
+    if (a.summary && !(m.status & (DHMC_CHAIN_BAD_STEPSIZE | DHMC_CHAIN_LEAPFROG_NONFINITE)))
+      summary_fold<DeviceBackend<EPL, FAM, W, DN, G, DP>>(a.summary, b.slot_tab, b.n_slots, b.tid, b.grp, a.D, summary_problem(a, c));
     if constexpr (G > 1) { if (a.pooled || a.batch_k) b.coop_finish(); }     // group fetch: the group leaves together, then the CTA takes the next one
   }
   b.coop_finish();

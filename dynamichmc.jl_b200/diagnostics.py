@@ -5,6 +5,8 @@ from dataclasses import dataclass
 
 import numpy as np
 
+from . import _lib as L
+
 ACCEPTANCE_QUANTILES = [0.05, 0.25, 0.5, 0.75, 0.95]      # diagnostics.jl:35
 
 
@@ -190,3 +192,110 @@ def ess_rhat(draws, max_lag=0):
         tau = max(tau, 1.0 / np.log10(m * n))
         ess[d] = m * n / tau
     return dict(rhat=rhat, ess=ess)
+
+
+# ------------------------------------------------------------------ streaming posterior summary
+# Numpy mirror of dhmc_mcmc_summary / dhmc_summary_merge / dhmc_summary_finish (include/dhmc.h, DESIGN.md §4.4): the
+# definitions the tests check the device against, and the merge path for shards gathered with torch.distributed.  A record
+# is [P, D, SUMMARY_FIELDS] (numpy order; the C ABI's column-major [F, D, P]) of mergeable quantities.
+def summary_from_draws(draws, chains_per_problem=0, thin=1, reference=None, chain_offset=0, n_problems=None,
+                       completed=None):
+    """The record dhmc_mcmc_summary folds on the device, from draws [K, N, D] of all N transitions (every thin-th is kept).
+    Chain k of this shard is global chain chain_offset + k and samples problem (chain_offset + k) // chains_per_problem
+    (chains_per_problem = 0: one problem).  `reference` [P, D] adds the rank counts; `completed` [K] (bool) leaves the
+    chains that failed out.  P defaults to reference's rows, else to the problems the shard reaches."""
+    from .api import _argcheck
+    x = np.asarray(draws, float)
+    _argcheck(x.ndim == 3, "draws: [chains, N, D]")
+    K, N, D = x.shape
+    _argcheck(thin >= 1 and N % thin == 0 and N // thin >= 4, "thin ≥ 1, N a multiple of thin, N / thin ≥ 4")
+    x = x[:, thin - 1::thin]
+    n_keep = x.shape[1]
+    n = n_keep // 2
+    cpp = int(chains_per_problem or 0)
+    if reference is not None:
+        reference = np.asarray(reference, float)
+        _argcheck(reference.ndim == 2 and reference.shape[1] == D, "reference: [P, D]")
+    if cpp:
+        P = int(n_problems if n_problems is not None else
+                reference.shape[0] if reference is not None else -(-(chain_offset + K) // cpp))
+        prob = (chain_offset + np.arange(K)) // cpp
+    else:
+        P, prob = 1, np.zeros(K, dtype=np.int64)
+    _argcheck(reference is None or reference.shape[0] == P, "reference: [P, D]")
+    ok = np.ones(K, bool) if completed is None else np.asarray(completed, bool)
+    rec = np.zeros((P, D, L.SUMMARY_FIELDS))
+    rec[..., L.SUMMARY_NKEEP] = n_keep
+    rec[..., L.SUMMARY_BELOW] = np.nan if reference is None else 0.0
+    for p in range(P):
+        idx = np.flatnonzero((prob == p) & ok)
+        M = idx.size
+        rec[p, :, L.SUMMARY_CHAINS] = M
+        if M == 0:
+            continue
+        s = x[idx[0], 0]                                                  # shift: everything below is relative to one draw,
+        seq = np.stack([x[idx, :n], x[idx, n:2 * n]], axis=1) - s         # so a large common offset cancels exactly [M, 2, n, D]
+        mu = seq.mean(axis=2)                                             # [M, 2, D] sequence means
+        mbar = mu.mean(axis=(0, 1))
+        muc = 0.5 * (mu[:, 0] + mu[:, 1])                                 # chain means over 2n draws
+        rec[p, :, L.SUMMARY_MEAN] = s + mbar
+        rec[p, :, L.SUMMARY_SS_SEQ] = ((mu - mbar) ** 2).sum(axis=(0, 1))
+        rec[p, :, L.SUMMARY_M2] = ((seq - mu[:, :, None]) ** 2).sum(axis=(0, 1, 2))
+        rec[p, :, L.SUMMARY_SS_CHAIN] = ((muc - mbar) ** 2).sum(axis=0)
+        if reference is not None:
+            rec[p, :, L.SUMMARY_BELOW] = (x[idx] < reference[p]).sum(axis=(0, 1))
+    return rec
+
+
+def merge_summaries(*records):
+    """dhmc_summary_merge over any number of records of the same [P, D]: the record of all their chains (Chan, Golub and
+    LeVeque's pairwise update of means and centred sums of squares; counts add)."""
+    from .api import _argcheck
+    out = np.array(records[0], float, copy=True)
+    for r in records[1:]:
+        r = np.asarray(r, float)
+        _argcheck(r.shape == out.shape, "records of the same [P, D]")
+        ma, mb = out[..., L.SUMMARY_CHAINS], r[..., L.SUMMARY_CHAINS]
+        both = (ma > 0) & (mb > 0)
+        _argcheck(np.all(out[..., L.SUMMARY_NKEEP][both] == r[..., L.SUMMARY_NKEEP][both]),
+                  "records of runs with the same number of kept draws per chain")
+        below = out[..., L.SUMMARY_BELOW] + r[..., L.SUMMARY_BELOW]
+        take = (ma == 0) & (mb > 0)
+        out[take] = r[take]
+        M = ma + mb
+        with np.errstate(invalid="ignore", divide="ignore"):
+            delta = r[..., L.SUMMARY_MEAN] - out[..., L.SUMMARY_MEAN]
+            mean = out[..., L.SUMMARY_MEAN] + delta * (mb / M)
+            ss = out[..., L.SUMMARY_SS_SEQ] + r[..., L.SUMMARY_SS_SEQ] + delta * delta * (2.0 * ma * mb / M)
+            ssc = out[..., L.SUMMARY_SS_CHAIN] + r[..., L.SUMMARY_SS_CHAIN] + delta * delta * (ma * mb / M)
+        out[..., L.SUMMARY_MEAN] = np.where(both, mean, out[..., L.SUMMARY_MEAN])
+        out[..., L.SUMMARY_SS_SEQ] = np.where(both, ss, out[..., L.SUMMARY_SS_SEQ])
+        out[..., L.SUMMARY_SS_CHAIN] = np.where(both, ssc, out[..., L.SUMMARY_SS_CHAIN])
+        out[..., L.SUMMARY_M2] = np.where(both, out[..., L.SUMMARY_M2] + r[..., L.SUMMARY_M2], out[..., L.SUMMARY_M2])
+        out[..., L.SUMMARY_CHAINS] = np.where(both, M, out[..., L.SUMMARY_CHAINS])
+        out[..., L.SUMMARY_BELOW] = below
+    return out
+
+
+def finish_summary(record):
+    """dhmc_summary_finish: mean, sd, mcse, ess, rhat [P, D] (float), rank and draws [P, D] (int64; rank −1 without a
+    reference) from a record.  Definitions in include/dhmc.h; ess is a between-chain batch-means estimate, not the Geyer
+    ESS of ess_rhat."""
+    r = np.asarray(record, float)
+    M = r[..., L.SUMMARY_CHAINS]
+    m, n = 2.0 * M, np.floor(r[..., L.SUMMARY_NKEEP] / 2.0)
+    ss, m2 = r[..., L.SUMMARY_SS_SEQ], r[..., L.SUMMARY_M2]
+    none = M == 0
+    with np.errstate(invalid="ignore", divide="ignore"):
+        var = (m2 + n * ss) / (m * n - 1.0)
+        W = m2 / (m * (n - 1.0))
+        var_plus = (n - 1.0) / n * W + ss / (m - 1.0)
+        var_c = r[..., L.SUMMARY_SS_CHAIN] / (M - 1.0) / M
+        out = dict(mean=np.where(none, np.nan, r[..., L.SUMMARY_MEAN]), sd=np.where(none, np.nan, np.sqrt(var)),
+                   rhat=np.where(none, np.nan, np.sqrt(var_plus / W)),
+                   mcse=np.where(M >= 2, np.sqrt(var_c), np.nan),
+                   ess=np.where((M >= 2) & (var_plus > 0), var / var_c, np.nan))
+    below = r[..., L.SUMMARY_BELOW]
+    out["rank"] = np.where(np.isnan(below), -1, np.nan_to_num(below)).astype(np.int64)
+    out["draws"] = (r[..., L.SUMMARY_NKEEP] * M).astype(np.int64)
+    return out

@@ -214,6 +214,51 @@ int dhmc_host_free(dhmc_handle* h, void* p);
 int dhmc_mcmc_dev(dhmc_handle* h, int32_t N, double* posterior, dhmc_tree_stats* stats,
                   double* logdens);
 
+/* ---- streaming posterior summary (DESIGN.md §4.4): sample without keeping draws ------------------------------------
+ * dhmc_mcmc_summary takes N transitions at the adapted (κ, ϵ), exactly as dhmc_mcmc does (same draws, same final state, same
+ * transition count, status words, return code), keeps every thin-th one and folds the kept draws into per-(problem,
+ * parameter) statistics on the device instead of writing them out.  Definitions: chain c keeps n_keep = N / thin draws;
+ * sequence 0 is the first n = ⌊n_keep/2⌋ of them, sequence 1 the next n (an odd n_keep drops its last draw from the
+ * moments).  Problem p (a handle without a batch is one problem, P = 1) pools its M local chains that completed the call,
+ * m = 2M sequences; a chain whose status has DHMC_CHAIN_BAD_STEPSIZE or DHMC_CHAIN_LEAPFROG_NONFINITE is left out.  Per
+ * parameter d:
+ *   mean   mean of the 2n·M draws (= the mean of the sequence means μ_s)
+ *   sd     √ of their pooled variance (Σ_s M2_s + n·Σ_s (μ_s − μ̄)²) / (m·n − 1)
+ *   rhat   split-R̂ as dhmc_ess_rhat_problems_dev: W = Σ_s M2_s / (m(n − 1)), var⁺ = (n − 1)/n·W + var(μ_s), √(var⁺ / W)
+ *   mcse   √(var(μ_c) / M), μ_c = chain c's mean over its 2n draws (between-chain batch means; NaN for M < 2)
+ *   ess    sd² / mcse² (NaN for M < 2 or var⁺ = 0).  A batch-means estimate that becomes precise with many chains, NOT the
+ *          Geyer ESS of dhmc_ess_rhat_dev.
+ *   rank   with a reference [D, P]: the number of the problem's kept draws (all n_keep of every local chain) with
+ *          θ_d < reference[d, p], an exact integer — the rank statistic of simulation-based calibration (−1 without one)
+ *   draws  n_keep·M, the rank's denominator
+ * A problem with no local chain gets NaN everywhere (rank 0, draws 0).  Quantiles are not computed.
+ *
+ * The record is [DHMC_SUMMARY_FIELDS, D, P] column-major (the fields of (d, p) at (p·D + d)·F) and holds mergeable
+ * quantities in absolute terms: the records of shards of one run (handles with different chain_offset, ranks) combine with
+ * dhmc_summary_merge into the record one handle holding every chain would produce, up to rounding. */
+enum {
+  DHMC_SUMMARY_CHAINS = 0,   /* M: chains that contributed */
+  DHMC_SUMMARY_NKEEP = 1,    /* n_keep: kept draws per chain */
+  DHMC_SUMMARY_MEAN = 2,     /* μ̄: mean of the sequence means */
+  DHMC_SUMMARY_SS_SEQ = 3,   /* Σ_s (μ_s − μ̄)² over the 2M sequences */
+  DHMC_SUMMARY_M2 = 4,       /* Σ_s M2_s: within-sequence sums of squared deviations */
+  DHMC_SUMMARY_SS_CHAIN = 5, /* Σ_c (μ_c − μ̄)² over the M chains */
+  DHMC_SUMMARY_BELOW = 6,    /* kept draws below the reference (exact integer; NaN without a reference) */
+  DHMC_SUMMARY_FIELDS = 7
+};
+/* reference: host [D, P] or NULL; record: host [DHMC_SUMMARY_FIELDS, D, P]; stats / logdens: host [N/thin, B] or NULL (the
+ * kept transitions, as dhmc_mcmc_thinned).  DHMC_EARG before anything runs for N < 1, thin < 1, N % thin ≠ 0,
+ * N / thin < 4 or record == NULL.  Device memory: one grow-only arena of 8·P·D + 3·D·(resident chain groups) + P doubles.
+ * On DHMC_ENUMERIC the record is still written, without the chains that failed. */
+int dhmc_mcmc_summary(dhmc_handle* h, int32_t N, int32_t thin, const double* reference, double* record,
+                      dhmc_tree_stats* stats, double* logdens);
+/* record ← record ⊕ other (both [DHMC_SUMMARY_FIELDS, D, P]; pairwise update of Chan, Golub and LeVeque).  DHMC_EARG (and
+ * nothing written) when a cell with chains on both sides has two different n_keep.  Pure host code. */
+int dhmc_summary_merge(double* record, const double* other, int64_t D, int64_t P);
+/* The statistics above from a record; outputs [D, P] column-major, each may be NULL.  Pure host code. */
+int dhmc_summary_finish(const double* record, int64_t D, int64_t P, double* mean, double* sd, double* mcse, double* ess,
+                        double* rhat, int64_t* rank, int64_t* draws);
+
 /* ---- diagnostics on device-resident statistics (§8f) ------------------------ */
 /* Diagnostics.summarize_tree_statistics / EBFMI (diagnostics.jl:29-32, 65-106) reduced on the
  * GPU over stats_dev [N,B] (DEVICE pointer, e.g. the buffer given to dhmc_mcmc_dev): pooled

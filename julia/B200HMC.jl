@@ -334,6 +334,37 @@ function ess_rhat_problems(h::Handle, draws_dev::Ptr{Float64}, N::Integer, P::In
     (; rhat, ess)
 end
 
+# ---- streaming posterior summary (dhmc_mcmc_summary, include/dhmc.h; DESIGN.md §4.4) ----------------------------------
+const SUMMARY_FIELDS = 7
+"""N transitions at the adapted (κ, ϵ), every `thin`-th folded on the device into per-(parameter, problem) statistics; no draw
+is returned.  `reference` [D, P] adds the SBC ranks.  Returns the mergeable record [SUMMARY_FIELDS, D, P] (merge shards with
+`summary_merge!`, finish with `summary_finish`)."""
+function mcmc_summary(h::Handle, N::Integer, P::Integer; thin::Integer = 1, reference = nothing)
+    record = Array{Float64}(undef, SUMMARY_FIELDS, h.D, P)
+    ref = reference === nothing ? C_NULL : convert(Matrix{Float64}, reference)
+    _ck(h, ccall((:dhmc_mcmc_summary, LIB), Cint, (Ptr{Cvoid}, Int32, Int32, Ptr{Float64}, Ptr{Float64}, Ptr{Cvoid}, Ptr{Float64}),
+                 h.ptr, N, thin, ref, record, C_NULL, C_NULL))
+    record
+end
+"record ← record ⊕ other (dhmc_summary_merge): the record of the chains of both"
+function summary_merge!(record::Array{Float64,3}, other::Array{Float64,3})
+    rc = ccall((:dhmc_summary_merge, LIB), Cint, (Ptr{Float64}, Ptr{Float64}, Int64, Int64),
+               record, other, size(record, 2), size(record, 3))
+    rc == 0 || throw(ArgumentError("records of different shapes or kept-draw counts"))
+    record
+end
+"mean, sd, mcse, ess (batch means), rhat (split-R̂), rank (−1 without a reference), draws: [D, P] each (dhmc_summary_finish)"
+function summary_finish(record::Array{Float64,3})
+    D, P = size(record, 2), size(record, 3)
+    mean, sd, mcse, ess, rhat = (Matrix{Float64}(undef, D, P) for _ in 1:5)
+    rank, draws = Matrix{Int64}(undef, D, P), Matrix{Int64}(undef, D, P)
+    rc = ccall((:dhmc_summary_finish, LIB), Cint,
+               (Ptr{Float64}, Int64, Int64, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Int64}, Ptr{Int64}),
+               record, D, P, mean, sd, mcse, ess, rhat, rank, draws)
+    rc == 0 || throw(ArgumentError("summary record"))
+    (; mean, sd, mcse, ess, rhat, rank, draws)
+end
+
 # ---- mcmc_steps / mcmc_next_step — src/mcmc.jl:335-351: stepwise sampling at the adapted (κ, ϵ) -----
 struct MCMCSteps; h::Handle; end
 mcmc_steps(h::Handle) = MCMCSteps(h)
