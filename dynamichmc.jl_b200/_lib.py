@@ -31,7 +31,8 @@ EXPORTS = [
     "dhmc_ess_rhat_dev", "dhmc_ess_rhat_problems_dev", "dhmc_acceptance_quantiles_dev", "dhmc_mcmc_thinned", "dhmc_host_alloc", "dhmc_host_free",
     "dhmc_comm_unique_id", "dhmc_comm_init", "dhmc_comm_destroy", "dhmc_allgather_dev",
     "dhmc_allgather_positions_dev", "dhmc_last_comm_ms",
-    "dhmc_mcmc_summary", "dhmc_summary_merge", "dhmc_summary_finish",
+    "dhmc_mcmc_summary", "dhmc_summary_merge", "dhmc_summary_finish", "dhmc_mcmc_summary_histogram",
+    "dhmc_histogram_quantiles",
 ]
 # streaming summary record (include/dhmc.h DHMC_SUMMARY_*): numpy [P, D, SUMMARY_FIELDS] = column-major [F, D, P]
 (SUMMARY_CHAINS, SUMMARY_NKEEP, SUMMARY_MEAN, SUMMARY_SS_SEQ, SUMMARY_M2, SUMMARY_SS_CHAIN, SUMMARY_BELOW,
@@ -73,6 +74,10 @@ def lib(path=None):
         so.dhmc_mcmc_summary.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         so.dhmc_summary_merge.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64]
         so.dhmc_summary_finish.argtypes = [C.c_void_p, C.c_int64, C.c_int64] + [C.c_void_p] * 7
+        so.dhmc_mcmc_summary_histogram.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                   C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        so.dhmc_histogram_quantiles.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_int64,
+                                                C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
         _libs[path] = so
     return so
 

@@ -689,7 +689,7 @@ class Engine:
                                              L.ptr(stats), L.ptr(ld)))
         return dict(posterior_matrix=post, tree_statistics=stats, logdensities=ld)
 
-    def mcmc_summary(self, N, thin=1, reference=None, stats=False):
+    def mcmc_summary(self, N, thin=1, reference=None, stats=False, quantiles=None, grid=None, bins=256):
         """N transitions as mcmc (same draws, same final state and transition count), every thin-th kept and folded on the
         device into per-(problem, parameter) statistics instead of being returned (dhmc_mcmc_summary, DESIGN §4.4).
         `reference` [P, D] adds the SBC rank of each reference value among its problem's kept draws.  Returns a dict of
@@ -697,7 +697,14 @@ class Engine:
         without a reference), draws — plus `record` [P, D, SUMMARY_FIELDS], the mergeable form (diagnostics.merge_summaries,
         dhmc_summary_merge), and with stats=True the kept transitions' tree_statistics and logdensities [K, N // thin].
         A chain that fails is left out of its problem's statistics; the call raises as mcmc does, and the exception's
-        debug_information["summary"] holds the summary of the other chains."""
+        debug_information["summary"] holds the summary of the other chains.
+
+        `quantiles` (probabilities in [0, 1]) with `grid` = (lo, hi), each [P, D], also counts the kept draws into `bins`
+        equal bins between lo and hi plus one tail bin on each side (dhmc_mcmc_summary_histogram) and adds `quantile`,
+        `quantile_lo`, `quantile_hi` [P, D, len(quantiles)] (the exact quantile of the kept draws lies in [quantile_lo,
+        quantile_hi]; diagnostics.histogram_quantiles), `histogram` [P, D, bins + 2] (exact counts: those of shards on one
+        grid add up), `grid` and `probs`."""
+        from . import diagnostics
         _argcheck(N >= 1 and thin >= 1 and N % thin == 0, "N ≥ 1, thin ≥ 1 and N a multiple of thin")
         _argcheck(N // thin >= 4, "at least 4 kept draws per chain (N / thin ≥ 4)")
         P = self.ℓ.n_problems if isinstance(self.ℓ, ProblemBatch) else 1
@@ -705,15 +712,35 @@ class Engine:
         if reference is not None:
             ref = np.ascontiguousarray(reference, float)
             _argcheck(ref.shape == (P, self.D), f"reference: [P, D] = ({P}, {self.D})")
+        _argcheck(quantiles is not None or grid is None, "grid without quantiles")
+        counts = None
+        if quantiles is not None:
+            probs = np.ascontiguousarray(np.atleast_1d(np.asarray(quantiles, float)))
+            _argcheck(probs.ndim == 1 and probs.size >= 1 and np.all((probs >= 0.0) & (probs <= 1.0)),
+                      "quantiles: probabilities in [0, 1]")
+            _argcheck(grid is not None and len(grid) == 2, "quantiles need grid = (lo, hi), each [P, D]")
+            lo, hi = diagnostics.check_grid(grid[0], grid[1], bins, (P, self.D))
+            bins = int(bins)
+            counts = np.zeros((P, self.D, bins + 2), np.int64)
         record = np.zeros((P, self.D, L.SUMMARY_FIELDS))
         n = N // thin
         st = np.zeros((self.K, n), dtype=L.tree_stats_dtype) if stats else None
         ld = np.empty((self.K, n)) if stats else None
-        rc = self._lib.dhmc_mcmc_summary(self._h, N, thin, L.ptr(ref), L.ptr(record), L.ptr(st), L.ptr(ld))
+        if counts is None:
+            rc = self._lib.dhmc_mcmc_summary(self._h, N, thin, L.ptr(ref), L.ptr(record), L.ptr(st), L.ptr(ld))
+        else:
+            rc = self._lib.dhmc_mcmc_summary_histogram(self._h, N, thin, L.ptr(ref), L.ptr(lo), L.ptr(hi), bins,
+                                                       L.ptr(record), L.ptr(counts), L.ptr(st), L.ptr(ld))
         if rc not in (L.DHMC_OK, L.DHMC_ENUMERIC):
             self._ck(rc)
         out = self.summary_finish(record)
         out["record"] = record
+        if counts is not None:
+            shape = (P, self.D, probs.size)
+            q, q_lo, q_hi = np.empty(shape), np.empty(shape), np.empty(shape)
+            self._ck(self._lib.dhmc_histogram_quantiles(L.ptr(counts), L.ptr(lo), L.ptr(hi), bins, self.D, P, L.ptr(probs),
+                                                        probs.size, L.ptr(q), L.ptr(q_lo), L.ptr(q_hi)))
+            out.update(quantile=q, quantile_lo=q_lo, quantile_hi=q_hi, histogram=counts, grid=(lo, hi), probs=probs)
         if stats:
             out.update(tree_statistics=st, logdensities=ld)
         try:
@@ -970,16 +997,27 @@ def mcmc_with_warmup(seed, ℓ, N, chains=None, initialization=None, warmup_stag
 
 
 def summarize_with_warmup(seed, ℓ, N, thin=1, reference=None, chains=None, initialization=None, warmup_stages=None,
-                          algorithm=None, device=0, chain_offset=0, engine_opts=None, reporter=None):
+                          algorithm=None, device=0, chain_offset=0, engine_opts=None, reporter=None, quantiles=None,
+                          grid=None, bins=256):
     """mcmc_with_warmup ending in Engine.mcmc_summary instead of Results: the warm-up, then N transitions whose every
     thin-th draw is folded on the device into per-(problem, parameter) mean, sd, mcse, ess, rhat and — with a reference
     [P, D] — SBC ranks.  Memory and traffic do not grow with N: simulation-based calibration over a ProblemBatch of
-    thousands of data sets is one call.  Returns the dict of Engine.mcmc_summary."""
+    thousands of data sets is one call.  Returns the dict of Engine.mcmc_summary.
+
+    `quantiles` adds bracketed quantiles on `bins` bins of `grid` = (lo, hi) [P, D] (Engine.mcmc_summary).  Without a grid,
+    a pilot fixes it: after the warm-up, mcmc_summary(max(4, N // 10)) runs as a last warm-up step and the grid is
+    diagnostics.quantile_grid of its summary, mean ± 6·sd per (problem, parameter).  The pilot's transitions come before
+    the N transitions of the summary (the chains go on from where the pilot left them)."""
+    from . import diagnostics
     chains = _default_chains(ℓ, chains, chain_offset)
     eng, _ = _warm_up(seed, ℓ, chains, initialization, warmup_stages, algorithm, False, device, chain_offset,
                       engine_opts, reporter)
     try:
-        out = eng.mcmc_summary(N, thin=thin, reference=reference)
+        if quantiles is not None and grid is None:
+            n_pilot = max(4, N // 10)
+            grid = diagnostics.quantile_grid(eng.mcmc_summary(n_pilot))
+            _report(reporter, "quantile grid pilot finished", transitions=n_pilot, chains=chains)
+        out = eng.mcmc_summary(N, thin=thin, reference=reference, quantiles=quantiles, grid=grid, bins=bins)
         _report(reporter, "inference finished", transitions=N, chains=chains)
     finally:
         eng.close()

@@ -21,6 +21,7 @@
 #include <pthread.h>
 #include <sched.h>
 
+#include <algorithm>
 #include <chrono>
 #include <cmath>
 #include <cstdio>
@@ -1385,9 +1386,22 @@ int dhmc_mcmc_dev(dhmc_handle* h, int32_t N, double* posterior, dhmc_tree_stats*
 // record [DHMC_SUMMARY_FIELDS, D, P] column-major: the fields of (parameter d, problem p) at (p·D + d)·F
 static double* summary_cell(double* record, int64_t D, int64_t p, int64_t d) { return record + ((size_t)p * D + d) * DHMC_SUMMARY_FIELDS; }
 
-int dhmc_mcmc_summary(dhmc_handle* h, int32_t N, int32_t thin, const double* reference, double* record, dhmc_tree_stats* stats,
-                      double* logdens) {
-  if (!h) return DHMC_EARG;
+// The grid of every (d, p) cell of a quantile histogram (include/dhmc.h): nbins in [1, 4096], lo < hi finite, hi − lo and
+// nbins / (hi − lo) finite (so that inv_w is a finite number)
+static bool valid_grid(const double* lo, const double* hi, int nbins, size_t cells) {
+  if (!lo || !hi || nbins < 1 || nbins > 4096) return false;
+  for (size_t i = 0; i < cells; ++i) {
+    const double w = hi[i] - lo[i];
+    if (!(std::isfinite(lo[i]) && std::isfinite(hi[i]) && lo[i] < hi[i] && std::isfinite(w) && std::isfinite((double)nbins / w)))
+      return false;
+  }
+  return true;
+}
+
+// dhmc_mcmc_summary and, with counts, dhmc_mcmc_summary_histogram (arguments checked by the caller)
+static int mcmc_summary(dhmc_handle* h, int32_t N, int32_t thin, const double* reference, const double* lo_host,
+                        const double* hi_host, int32_t nbins, double* record, int64_t* counts, dhmc_tree_stats* stats,
+                        double* logdens) {
   if (N < 1 || thin < 1 || N % thin != 0) { h->err = "dhmc_mcmc_summary: N ≥ 1, thin ≥ 1 and N a multiple of thin"; return DHMC_EARG; }
   const int n_keep = N / thin;
   if (n_keep < 4) { h->err = "dhmc_mcmc_summary: at least 4 kept draws per chain (N / thin ≥ 4)"; return DHMC_EARG; }
@@ -1397,9 +1411,11 @@ int dhmc_mcmc_summary(dhmc_handle* h, int32_t N, int32_t thin, const double* ref
   const size_t D = (size_t)h->cfg.dim, B = (size_t)h->cfg.n_chains;
   const int64_t K = h->batch_k, off = h->cfg.chain_offset;
   const size_t P = K ? (size_t)h->batch_p : 1, PD = P * D, rows = (size_t)h->grid * h->G * 3 * D;
-  // one grow-only arena, 8-byte elements throughout: acc [P][5][D], shift [P][D], ref [P][D], row [grid·G][3][D],
-  // below [P][D], chains [P]
-  const size_t need = sizeof(double) * (8 * PD + rows + P);
+  // histograms (counts != NULL): cells bins per (d, p); the staging rows of the resident chain groups
+  const size_t cells = counts ? (size_t)nbins + 2 : 0, stage = (size_t)h->grid * h->G * cells * D;
+  // one grow-only arena: acc [P][5][D], shift [P][D], ref [P][D], row [grid·G][3][D], below [P][D], chains [P], then with
+  // histograms hist [P][D][cells], lo [P][D], inv_w [P][D] (8-byte elements) and stage [grid·G][cells][D] (4-byte)
+  const size_t need = sizeof(double) * (8 * PD + rows + P + PD * cells + (counts ? 2 * PD : 0)) + sizeof(unsigned) * stage;
   if (need > h->sum_bytes) {
     cudaFree(h->sum_buf); h->sum_buf = nullptr; h->sum_bytes = 0;
     CK(cudaMalloc(&h->sum_buf, need));
@@ -1423,7 +1439,18 @@ int dhmc_mcmc_summary(dhmc_handle* h, int32_t N, int32_t thin, const double* ref
   if (p1 >= pa)
     CK(cudaMemcpy2DAsync(shift + pa * D, sizeof(double) * D, h->q + (size_t)(K ? pa * K - off : 0) * D, sizeof(double) * D * (size_t)(K ? K : 1),
                          sizeof(double) * D, (size_t)(p1 - pa + 1), cudaMemcpyDeviceToDevice, h->stream));
-  const SummaryArgs sa{row, shift, reference ? ref : nullptr, acc, below, chains, n_keep / 2};
+  SummaryArgs sa{row, shift, reference ? ref : nullptr, acc, below, chains, n_keep / 2, nullptr, nullptr, nullptr, nullptr, 0};
+  if (counts) {
+    unsigned long long* hist = chains + P;
+    double* lo = (double*)(hist + PD * cells);
+    double* inv_w = lo + PD;
+    std::vector<double> hinv(PD);
+    for (size_t i = 0; i < PD; ++i) hinv[i] = (double)nbins / (hi_host[i] - lo_host[i]);
+    CK(cudaMemsetAsync(hist, 0, sizeof(unsigned long long) * PD * cells, h->stream));
+    CK(cudaMemcpyAsync(lo, lo_host, sizeof(double) * PD, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(inv_w, hinv.data(), sizeof(double) * PD, cudaMemcpyHostToDevice, h->stream));
+    sa.lo = lo; sa.inv_w = inv_w; sa.stage = (unsigned*)(inv_w + PD); sa.hist = hist; sa.nbins = nbins;
+  }
   CK(cudaMemcpyAsync(h->sum_args, &sa, sizeof sa, cudaMemcpyHostToDevice, h->stream));
   AdaptConfig cfg{};
   const int rc = run_nuts(h, N, cfg, 0.0, nullptr, nullptr, nullptr, stats, nullptr, logdens, false, true, nullptr, thin, false,
@@ -1434,6 +1461,8 @@ int dhmc_mcmc_summary(dhmc_handle* h, int32_t N, int32_t thin, const double* ref
   CK(cudaMemcpyAsync(hacc.data(), acc, sizeof(double) * hacc.size(), cudaMemcpyDeviceToHost, h->stream));
   CK(cudaMemcpyAsync(hshift.data(), shift, sizeof(double) * PD, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaMemcpyAsync(hcnt.data(), below, sizeof(unsigned long long) * hcnt.size(), cudaMemcpyDeviceToHost, h->stream));
+  if (counts)        // [P][D][cells] is the column-major [cells, D, P] of the ABI; uint64 counts stay far below 2^63
+    CK(cudaMemcpyAsync(counts, below + PD + P, sizeof(int64_t) * PD * cells, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   for (size_t p = 0; p < P; ++p) {
     const double M = (double)hcnt[PD + p], m = 2.0 * M;
@@ -1455,6 +1484,77 @@ int dhmc_mcmc_summary(dhmc_handle* h, int32_t N, int32_t thin, const double* ref
     }
   }
   return rc;
+}
+
+int dhmc_mcmc_summary(dhmc_handle* h, int32_t N, int32_t thin, const double* reference, double* record, dhmc_tree_stats* stats,
+                      double* logdens) {
+  if (!h) return DHMC_EARG;
+  return mcmc_summary(h, N, thin, reference, nullptr, nullptr, 0, record, nullptr, stats, logdens);
+}
+
+int dhmc_mcmc_summary_histogram(dhmc_handle* h, int32_t N, int32_t thin, const double* reference, const double* lo,
+                                const double* hi, int32_t nbins, double* record, int64_t* counts, dhmc_tree_stats* stats,
+                                double* logdens) {
+  if (!h) return DHMC_EARG;
+  if (!counts) { h->err = "dhmc_mcmc_summary_histogram: counts is NULL"; return DHMC_EARG; }
+  const size_t cells = (size_t)h->cfg.dim * (h->batch_k ? (size_t)h->batch_p : 1);
+  if (!valid_grid(lo, hi, nbins, cells)) {
+    h->err = "dhmc_mcmc_summary_histogram: 1 ≤ nbins ≤ 4096 and, per cell, finite lo < hi with hi − lo and nbins / (hi − lo) finite";
+    return DHMC_EARG;
+  }
+  return mcmc_summary(h, N, thin, reference, lo, hi, nbins, record, counts, stats, logdens);
+}
+
+// Type-7 quantile (Julia's default) at α of the values counted in bins 0 … nbins + 1 on the grid (lo, hi, nbins), as
+// include/dhmc.h defines it: cum[k] = C_k, the count of bins 0 … k.  Order statistic r lies in the first bin k with r < C_k
+// and is placed strictly inside it, at e_{k−1} + ((r − C_{k−1}) + 0.5)/c_k · (e_k − e_{k−1}).  Shared by
+// dhmc_histogram_quantiles and dhmc_acceptance_quantiles_dev, whose grid (0, 1, 4096) has exact edges.
+static void binned_quantile(const unsigned long long* cum, int nbins, double lo, double hi, double alpha, double* q, double* q_lo,
+                            double* q_hi) {
+  const unsigned long long n = cum[nbins + 1];
+  if (n == 0) { *q = *q_lo = *q_hi = dm_nan(); return; }
+  const double w = (hi - lo) / (double)nbins;
+  auto edge = [&](int k) { return k < nbins ? lo + (double)k * w : hi; };
+  auto bin_of = [&](unsigned long long r) { return (int)(std::upper_bound(cum, cum + nbins + 2, r) - cum); };
+  auto place = [&](unsigned long long r, int k) {
+    if (k == 0 || k == nbins + 1) return dm_nan();
+    const unsigned long long below = cum[k - 1];
+    return edge(k - 1) + ((double)(r - below) + 0.5) / (double)(cum[k] - below) * (edge(k) - edge(k - 1));
+  };
+  const double pos = alpha * (double)(n - 1);
+  const unsigned long long j = (unsigned long long)pos;
+  const double gamma = pos - (double)j;
+  const int kj = bin_of(j), kh = gamma > 0.0 ? bin_of(j + 1) : kj;
+  const double xj = place(j, kj);
+  *q = gamma > 0.0 ? xj + gamma * (place(j + 1, kh) - xj) : xj;
+  *q_lo = kj == 0 ? -dm_inf() : edge(kj - 1);
+  *q_hi = kh == nbins + 1 ? dm_inf() : edge(kh);
+}
+
+int dhmc_histogram_quantiles(const int64_t* counts, const double* lo, const double* hi, int32_t nbins, int64_t D, int64_t P,
+                             const double* probs, int32_t nprobs, double* q, double* q_lo, double* q_hi) {
+  if (!counts || !probs || D < 1 || P < 1 || nprobs < 1) return DHMC_EARG;
+  const size_t n_cells = (size_t)D * (size_t)P;
+  if (!valid_grid(lo, hi, nbins, n_cells)) return DHMC_EARG;
+  for (int k = 0; k < nprobs; ++k)
+    if (!(probs[k] >= 0.0 && probs[k] <= 1.0)) return DHMC_EARG;
+  const size_t nb2 = (size_t)nbins + 2;
+  for (size_t i = 0; i < n_cells * nb2; ++i)
+    if (counts[i] < 0) return DHMC_EARG;
+  std::vector<unsigned long long> cum(nb2);
+  for (size_t i = 0; i < n_cells; ++i) {
+    unsigned long long c = 0;
+    for (size_t b = 0; b < nb2; ++b) cum[b] = c += (unsigned long long)counts[i * nb2 + b];
+    for (int k = 0; k < nprobs; ++k) {
+      double a, l, u;
+      binned_quantile(cum.data(), nbins, lo[i], hi[i], probs[k], &a, &l, &u);
+      const size_t o = i * (size_t)nprobs + k;
+      if (q) q[o] = a;
+      if (q_lo) q_lo[o] = l;
+      if (q_hi) q_hi[o] = u;
+    }
+  }
+  return DHMC_OK;
 }
 
 int dhmc_summary_merge(double* record, const double* other, int64_t D, int64_t P) {
@@ -1631,25 +1731,15 @@ int dhmc_acceptance_quantiles_dev(dhmc_handle* h, const dhmc_tree_stats* stats_d
   if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
   cudaFree(d_hist);
   if (e != cudaSuccess) { h->err = cudaGetErrorString(e); return DHMC_ECUDA; }
-  const unsigned long long tot = n - hist[BINS];
-  // order statistic j (0-based) of the non-NaN rates, placed by its rank among the records of its bin: strictly inside
-  // the bin, so less than one bin width from the true value
-  auto order_stat = [&](unsigned long long j) {
-    unsigned long long cum = 0;
-    for (int b = 0; b < BINS; ++b) {
-      if (j < cum + hist[b]) return ((double)b + ((double)(j - cum) + 0.5) / (double)hist[b]) / BINS;
-      cum += hist[b];
-    }
-    return 1.0;
-  };
+  // the non-NaN rates in bins 1 … BINS of the grid (0, 1, BINS), both tails empty: every order statistic is placed
+  // strictly inside its bin, so less than one bin width from the true value
+  std::vector<unsigned long long> cum(BINS + 2, 0);
+  for (int b = 0; b < BINS; ++b) cum[b + 1] = cum[b] + hist[b];
+  cum[BINS + 1] = cum[BINS];
   for (int k = 0; k < nprobs; ++k) {
     if (!(probs[k] >= 0.0 && probs[k] <= 1.0)) { h->err = "0 ≤ p ≤ 1"; return DHMC_EARG; }
-    if (tot == 0) { out[k] = dm_nan(); continue; }
-    // Julia's quantile (type 7): x₍ⱼ₎ + γ (x₍ⱼ₊₁₎ − x₍ⱼ₎) at position p (n − 1) = j + γ of the sorted sample
-    const double pos = probs[k] * (double)(tot - 1);
-    const unsigned long long j = (unsigned long long)pos;
-    const double gamma = pos - (double)j, lo = order_stat(j);
-    out[k] = gamma > 0.0 ? lo + gamma * (order_stat(j + 1) - lo) : lo;
+    double q_lo, q_hi;
+    binned_quantile(cum.data(), BINS, 0.0, 1.0, probs[k], out + k, &q_lo, &q_hi);
   }
   return DHMC_OK;
 }

@@ -39,6 +39,10 @@ struct ProblemDesc {
 //   acc    [P][5][D]       Σ(μ_s − s), Σ(μ_s − s)², Σ M2_s over sequences; Σ(μ_c − s), Σ(μ_c − s)² over chains
 //   below  [P][D]          Σ #{kept draws with θ < reference} (exact)
 //   chains [P]             chains that completed the call
+// Histograms for quantiles (dhmc_mcmc_summary_histogram; hist null: off), nbins + 2 bins per cell (include/dhmc.h):
+//   lo, inv_w [P][D]                 the grid: lower end and nbins / (hi − lo)
+//   stage [grid·G][nbins + 2][D]     per chain group: the counts of the running chain (cleared at its first kept draw)
+//   hist  [P][D][nbins + 2]          Σ over the problem's completed chains (the host layout)
 struct SummaryArgs {
   double* row;
   const double* shift;
@@ -47,6 +51,11 @@ struct SummaryArgs {
   unsigned long long* below;
   unsigned long long* chains;
   int n;                        // draws per sequence: ⌊N_keep / 2⌋
+  const double* lo;
+  const double* inv_w;
+  unsigned* stage;
+  unsigned long long* hist;
+  int nbins;
 };
 
 struct KArgs {
@@ -296,9 +305,59 @@ __device__ __forceinline__ Bk welford_view(double** slot_tab, int n_slots, int t
   return w;
 }
 template <class Bk>
+__device__ __forceinline__ size_t summary_group(int grp) {
+  return Bk::G > 1 ? (size_t)blockIdx.x * Bk::G + grp : (size_t)blockIdx.x;
+}
+template <class Bk>
 __device__ __forceinline__ double* summary_row(const SummaryArgs& s, int grp, int D) {
-  const size_t group = Bk::G > 1 ? (size_t)blockIdx.x * Bk::G + grp : (size_t)blockIdx.x;
-  return s.row + group * 3 * (size_t)D;
+  return s.row + summary_group<Bk>(grp) * 3 * (size_t)D;
+}
+template <class Bk>
+__device__ __forceinline__ unsigned* summary_stage(const SummaryArgs& s, int grp, int D) {
+  return s.stage + summary_group<Bk>(grp) * (size_t)(s.nbins + 2) * (size_t)D;
+}
+// Quantile histograms (include/dhmc.h): out of line again, with rolled loops that re-read the kept position from its slot
+// (zq: the thread's first element, element e at zq[e·T]).  ptxas allocates k_nuts' registers together with these bodies,
+// so they stay small, and the summary functions' own element loops are rolled too: with them unrolled, plain sampling in
+// some dense-metric kernels slowed by 11 – 12 % (benchmarks/streaming_quantiles_ptxas.md).  Kept draw j: the thread clears its own staging cells at j = 0 and adds
+// one count per element; the bin rule rounds the subtract and the multiply apart.
+template <class Bk>
+__device__ __noinline__ void summary_hist_draw(const SummaryArgs* sp, const double* zq, int tid, int grp, int D, size_t p, int j) {
+  constexpr int EPL = sizeof(Bk::q) / sizeof(double), T = Bk::T;
+  const SummaryArgs& s = *sp;
+  const int nb = s.nbins;
+  unsigned* stage = summary_stage<Bk>(s, grp, D);
+#pragma unroll 1
+  for (int e = 0; e < EPL; ++e) {
+    const int i = tid + e * T;
+    if (i >= D) break;
+    if (j == 0) {
+#pragma unroll 1
+      for (int k = 0; k < nb + 2; ++k) stage[(size_t)k * D + i] = 0u;
+    }
+    const double t = __dmul_rn(__dsub_rn(zq[e * T], s.lo[p * D + i]), s.inv_w[p * D + i]);
+    const int k = t < 0.0 ? 0 : !(t < (double)nb) ? nb + 1 : 1 + (int)t;
+    stage[(size_t)k * D + i] += 1u;
+  }
+}
+// chain end (completed chains only): the non-zero staging cells into the problem's histogram
+template <class Bk>
+__device__ __noinline__ void summary_hist_fold(const SummaryArgs* sp, int tid, int grp, int D, size_t p) {
+  constexpr int EPL = sizeof(Bk::q) / sizeof(double), T = Bk::T;
+  const SummaryArgs& s = *sp;
+  const size_t cells = (size_t)s.nbins + 2;
+  const unsigned* stage = summary_stage<Bk>(s, grp, D);
+#pragma unroll 1
+  for (int e = 0; e < EPL; ++e) {
+    const int i = tid + e * T;
+    if (i >= D) break;
+    unsigned long long* hist = s.hist + (p * D + i) * cells;
+#pragma unroll 1
+    for (size_t k = 0; k < cells; ++k) {
+      const unsigned c = stage[k * D + i];
+      if (c) atomicAdd(hist + k, (unsigned long long)c);
+    }
+  }
 }
 // kept draw j: sequence 0 is draws [0, n), sequence 1 draws [n, 2n); an odd last draw counts for the rank only
 template <class Bk>
@@ -326,15 +385,17 @@ __device__ __noinline__ void summary_draw(const SummaryArgs* sp, double** slot_t
   }
   if (s.ref) {
     const double* ref = s.ref + p * D;
-#pragma unroll
+    const double* zq = slot_tab[s_zq] + tid;
+#pragma unroll 1
     for (int e = 0; e < EPL; ++e) {
       const int i = tid + e * T;
       if (i < D) {
-        const double below = w.q[e] < ref[i] ? 1.0 : 0.0;
+        const double below = zq[e * T] < ref[i] ? 1.0 : 0.0;
         row[2 * D + i] = j == 0 ? below : row[2 * D + i] + below;
       }
     }
   }
+  if (s.hist) summary_hist_draw<Bk>(sp, slot_tab[s_zq] + tid, tid, grp, D, p, j);
 }
 // chain end (the chain completed the call): fold its two sequences into its problem's sums
 template <class Bk>
@@ -346,7 +407,7 @@ __device__ __noinline__ void summary_fold(const SummaryArgs* sp, double** slot_t
   const double* sv = slot_tab[n_slots - 2] + tid;
   const size_t D = (size_t)Di;
   double* acc = s.acc + p * 5 * D;
-#pragma unroll
+#pragma unroll 1
   for (int e = 0; e < EPL; ++e) {
     const int i = tid + e * T;
     if (i < Di) {
@@ -360,6 +421,7 @@ __device__ __noinline__ void summary_fold(const SummaryArgs* sp, double** slot_t
       if (s.ref) atomicAdd(s.below + p * D + i, (unsigned long long)row[2 * D + i]);
     }
   }
+  if (s.hist) summary_hist_fold<Bk>(sp, tid, grp, Di, p);
   if (tid == 0) atomicAdd(s.chains + p, 1ull);
 }
 

@@ -299,3 +299,123 @@ def finish_summary(record):
     out["rank"] = np.where(np.isnan(below), -1, np.nan_to_num(below)).astype(np.int64)
     out["draws"] = (r[..., L.SUMMARY_NKEEP] * M).astype(np.int64)
     return out
+
+
+# ------------------------------------------------------------------ streaming quantiles
+# Numpy mirror of dhmc_mcmc_summary_histogram's bin counts and of dhmc_histogram_quantiles (include/dhmc.h, DESIGN.md §4.4):
+# the same IEEE operations in the same order, so counts agree as integers and quantiles bit for bit.  Counts are
+# [P, D, bins + 2] int64 (numpy order; the C ABI's column-major [bins + 2, D, P]); bin 0 is below lo, bin bins + 1 at or
+# above hi (and NaN).
+MAX_BINS = 4096
+
+
+def check_grid(lo, hi, bins, shape=None):
+    """(lo, hi) as float arrays [P, D] after the checks of the C ABI: 1 ≤ bins ≤ 4096 and, per cell, finite lo < hi with
+    hi − lo and bins / (hi − lo) finite."""
+    from .api import _argcheck
+    lo, hi = np.ascontiguousarray(lo, float), np.ascontiguousarray(hi, float)
+    _argcheck(lo.ndim == 2 and lo.shape == hi.shape and (shape is None or lo.shape == tuple(shape)),
+              f"grid: lo and hi of shape [P, D]{'' if shape is None else ' = ' + str(tuple(shape))}")
+    _argcheck(int(bins) == bins and 1 <= bins <= MAX_BINS, f"bins: 1 … {MAX_BINS}")
+    with np.errstate(over="ignore", invalid="ignore", divide="ignore"):
+        w = hi - lo
+        ok = np.isfinite(lo) & np.isfinite(hi) & (lo < hi) & np.isfinite(w) & np.isfinite(float(bins) / w)
+    _argcheck(bool(np.all(ok)), "grid: finite lo < hi with hi − lo and bins / (hi − lo) finite in every cell")
+    return lo, hi
+
+
+def histogram_from_draws(draws, lo, hi, bins, chains_per_problem=0, thin=1, chain_offset=0, n_problems=None,
+                         completed=None):
+    """The bin counts [P, D, bins + 2] dhmc_mcmc_summary_histogram folds on the device, from draws [K, N, D] of all N
+    transitions (every thin-th is kept), on the grid lo, hi [P, D].  Chains and problems as summary_from_draws; `completed`
+    [K] (bool) leaves the chains that failed out.  P is the grid's number of rows."""
+    from .api import _argcheck
+    x = np.asarray(draws, float)
+    _argcheck(x.ndim == 3, "draws: [chains, N, D]")
+    K, N, D = x.shape
+    _argcheck(thin >= 1 and N % thin == 0 and N // thin >= 4, "thin ≥ 1, N a multiple of thin, N / thin ≥ 4")
+    lo, hi = check_grid(lo, hi, bins)
+    bins = int(bins)
+    P = lo.shape[0]
+    _argcheck(lo.shape[1] == D and (n_problems is None or n_problems == P), "grid: [P, D]")
+    x = x[:, thin - 1::thin]
+    cpp = int(chains_per_problem or 0)
+    prob = (chain_offset + np.arange(K)) // cpp if cpp else np.zeros(K, dtype=np.int64)
+    ok = np.ones(K, bool) if completed is None else np.asarray(completed, bool)
+    inv_w = float(bins) / (hi - lo)
+    cells = bins + 2
+    counts = np.zeros((P, D, cells), np.int64)
+    for p in range(P):
+        xs = x[(prob == p) & ok]                                            # [M, n_keep, D]
+        with np.errstate(invalid="ignore", over="ignore"):
+            t = (xs - lo[p]) * inv_w[p]                                     # rounded apart, as on the device
+            inside = (t >= 0.0) & (t < bins)
+        k = np.where(t < 0.0, 0, bins + 1)
+        k[inside] = 1 + t[inside].astype(np.int64)
+        flat = (k + cells * np.arange(D)).ravel()
+        counts[p] = np.bincount(flat, minlength=D * cells).reshape(D, cells)
+    return counts
+
+
+def histogram_quantiles(counts, lo, hi, probs):
+    """dhmc_histogram_quantiles: (q, q_lo, q_hi), each [P, D, len(probs)], of counts [P, D, bins + 2] on the grid lo, hi
+    [P, D].  q is the type-7 quantile of the in-bin placements of the order statistics (NaN when one lies in a tail bin);
+    the exact type-7 quantile of the counted values lies in [q_lo, q_hi] up to the rounding of the edges."""
+    from .api import _argcheck
+    c = np.asarray(counts)
+    _argcheck(c.ndim == 3 and c.shape[2] >= 3 and np.issubdtype(c.dtype, np.integer) and np.all(c >= 0),
+              "counts: [P, D, bins + 2] of non-negative integers")
+    nb = c.shape[2] - 2
+    lo, hi = check_grid(lo, hi, nb, c.shape[:2])
+    probs = np.atleast_1d(np.asarray(probs, float))
+    _argcheck(probs.ndim == 1 and np.all((probs >= 0.0) & (probs <= 1.0)), "0 ≤ p ≤ 1")
+    cum = np.cumsum(c.astype(np.int64), axis=-1)
+    n = cum[..., -1]
+    w = (hi - lo) / float(nb)
+
+    def edge(k):
+        return np.where(k < nb, lo + k.astype(float) * w, hi)
+
+    def bin_of(r):                                                          # the first bin k with r < C_k
+        return (cum <= r[..., None]).sum(axis=-1)
+
+    def place(r, k):
+        kk = np.clip(k, 1, nb)
+        below = np.take_along_axis(cum, (kk - 1)[..., None], -1)[..., 0]
+        ck = np.take_along_axis(cum, kk[..., None], -1)[..., 0] - below
+        with np.errstate(invalid="ignore", divide="ignore"):
+            x = edge(kk - 1) + ((r - below).astype(float) + 0.5) / ck.astype(float) * (edge(kk) - edge(kk - 1))
+        return np.where((k == 0) | (k == nb + 1), np.nan, x)
+
+    shape = (*c.shape[:2], probs.size)
+    q, q_lo, q_hi = np.empty(shape), np.empty(shape), np.empty(shape)
+    empty = n == 0
+    for i, alpha in enumerate(probs):
+        pos = alpha * np.maximum(n - 1, 0).astype(float)
+        j = pos.astype(np.int64)
+        gamma = pos - j.astype(float)
+        kj = bin_of(j)
+        kh = np.where(gamma > 0.0, bin_of(j + 1), kj)
+        xj = place(j, kj)
+        with np.errstate(invalid="ignore"):
+            qi = np.where(gamma > 0.0, xj + gamma * (place(j + 1, kh) - xj), xj)
+        q[..., i] = np.where(empty, np.nan, qi)
+        q_lo[..., i] = np.where(empty, np.nan, np.where(kj == 0, -np.inf, edge(np.maximum(kj - 1, 0))))
+        q_hi[..., i] = np.where(empty, np.nan, np.where(kh == nb + 1, np.inf, edge(np.minimum(kh, nb))))
+    return q, q_lo, q_hi
+
+
+def quantile_grid(summary, width=6.0):
+    """The pilot grid of summarize_with_warmup: lo, hi [P, D] = mean ∓ width·sd per (problem, parameter), from a summary
+    (the dict of Engine.mcmc_summary / finish_summary) or a record [P, D, SUMMARY_FIELDS] (merged pilot records of shards
+    give every rank the same grid).  A cell whose mean ± width·sd is not a valid grid (sd = 0, sd not finite, no chain)
+    gets (c − s, c + s): c the mean (0 where it is not finite or |mean| > 1e300), s = max(1, |c|)."""
+    s = summary if isinstance(summary, dict) else finish_summary(summary)
+    mean, sd = np.asarray(s["mean"], float), np.asarray(s["sd"], float)
+    with np.errstate(over="ignore", invalid="ignore", divide="ignore"):
+        lo, hi = mean - width * sd, mean + width * sd
+        w = hi - lo
+        ok = np.isfinite(lo) & np.isfinite(hi) & (lo < hi) & np.isfinite(w) & np.isfinite(float(MAX_BINS) / w)
+    c = np.where(np.isfinite(mean) & (np.abs(mean) <= 1e300), mean, 0.0)
+    half = np.maximum(1.0, np.abs(c))
+    return np.where(ok, lo, c - half), np.where(ok, hi, c + half)

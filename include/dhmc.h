@@ -231,7 +231,7 @@ int dhmc_mcmc_dev(dhmc_handle* h, int32_t N, double* posterior, dhmc_tree_stats*
  *   rank   with a reference [D, P]: the number of the problem's kept draws (all n_keep of every local chain) with
  *          θ_d < reference[d, p], an exact integer — the rank statistic of simulation-based calibration (−1 without one)
  *   draws  n_keep·M, the rank's denominator
- * A problem with no local chain gets NaN everywhere (rank 0, draws 0).  Quantiles are not computed.
+ * A problem with no local chain gets NaN everywhere (rank 0, draws 0).  Quantiles: dhmc_mcmc_summary_histogram below.
  *
  * The record is [DHMC_SUMMARY_FIELDS, D, P] column-major (the fields of (d, p) at (p·D + d)·F) and holds mergeable
  * quantities in absolute terms: the records of shards of one run (handles with different chain_offset, ranks) combine with
@@ -258,6 +258,47 @@ int dhmc_summary_merge(double* record, const double* other, int64_t D, int64_t P
 /* The statistics above from a record; outputs [D, P] column-major, each may be NULL.  Pure host code. */
 int dhmc_summary_finish(const double* record, int64_t D, int64_t P, double* mean, double* sd, double* mcse, double* ess,
                         double* rhat, int64_t* rank, int64_t* draws);
+
+/* ---- streaming quantiles: per-(parameter, problem) histograms on a grid the caller fixes (DESIGN.md §4.4) ------------
+ * Exact quantiles do not stream in fixed memory; exact bin counts do, and they bracket every quantile.  The grid of
+ * (parameter d, problem p) is lo < hi, both finite, with hi − lo and nbins / (hi − lo) finite, 1 ≤ nbins ≤ 4096.  A kept
+ * draw θ goes into one of nbins + 2 bins, evaluated on the device and by the numpy mirror with the same IEEE operations
+ * (a separate subtract and multiply, no fused multiply-add):
+ *   inv_w = nbins / (hi − lo)            (once, on the host)
+ *   t     = (θ − lo) · inv_w
+ *   bin   = 0              if t < 0         (below lo)
+ *           nbins + 1      if !(t < nbins)  (at or above hi; NaN lands here too)
+ *           1 + (int)t     otherwise
+ * The histogram counts exactly the draws the rank counts: all n_keep kept draws of every local chain of problem p that
+ * completed the call (an odd last draw included), so Σ over bins = draws[d, p]; a chain with DHMC_CHAIN_BAD_STEPSIZE or
+ * DHMC_CHAIN_LEAPFROG_NONFINITE contributes nothing, even when it halted after keeping draws.  counts [nbins + 2, D, P]
+ * column-major (bin fastest) are exact integers: the histograms of shards of one run on one grid add up to the histogram
+ * of all their chains, so merging is adding the counts (no merge function is needed).
+ *
+ * Quantiles from the counts.  Edges e_k = lo + k·((hi − lo)/nbins) for k < nbins, e_nbins = hi.  For α ∈ [0, 1] and
+ * n = Σ counts: h = α(n − 1), j = ⌊h⌋, γ = h − j (Julia's type 7).  Order statistic r (0-based) lies in the bin k whose
+ * cumulative counts satisfy C_{k−1} ≤ r < C_k.
+ *   q_lo  the lower edge of the bin of r = j (−∞ for bin 0)
+ *   q_hi  the upper edge of the bin of r = j + 1 (r = j when γ = 0; +∞ for bin nbins + 1)
+ *   q     type-7 interpolation of the in-bin placements e_{k−1} + ((r − C_{k−1}) + 0.5)/c_k · (e_k − e_{k−1}) of the order
+ *         statistics it needs (dhmc_acceptance_quantiles_dev places its order statistics alike); NaN when one of them
+ *         lies in a tail bin
+ * n = 0 gives NaN for all three.  Guarantee: the exact type-7 quantile of the counted draws lies in [q_lo, q_hi], up to
+ * the rounding of the edges (a few ulps of max(|lo|, |hi|)).
+ *
+ * dhmc_mcmc_summary_histogram is dhmc_mcmc_summary (same draws, final state, transition count, status words, return code
+ * and record) that also writes counts.  lo, hi: host [D, P]; counts: host int64 [nbins + 2, D, P].  DHMC_EARG before
+ * anything runs for an invalid grid or nbins, counts == NULL, or any argument dhmc_mcmc_summary rejects.  Device memory
+ * on top of dhmc_mcmc_summary's arena: 8·P·D·(nbins + 4) + 4·D·(nbins + 2)·(resident chain groups) bytes (the problem
+ * histograms and the grid, and a staging histogram per resident chain group). */
+int dhmc_mcmc_summary_histogram(dhmc_handle* h, int32_t N, int32_t thin, const double* reference, const double* lo,
+                                const double* hi, int32_t nbins, double* record, int64_t* counts, dhmc_tree_stats* stats,
+                                double* logdens);
+/* q, q_lo, q_hi [nprobs, D, P] column-major (each may be NULL) of counts [nbins + 2, D, P] on the grid (lo, hi, nbins), as
+ * defined above.  DHMC_EARG for a probability outside [0, 1], an invalid grid, a negative count or a NULL input.  Pure
+ * host code. */
+int dhmc_histogram_quantiles(const int64_t* counts, const double* lo, const double* hi, int32_t nbins, int64_t D, int64_t P,
+                             const double* probs, int32_t nprobs, double* q, double* q_lo, double* q_hi);
 
 /* ---- diagnostics on device-resident statistics (§8f) ------------------------ */
 /* Diagnostics.summarize_tree_statistics / EBFMI (diagnostics.jl:29-32, 65-106) reduced on the

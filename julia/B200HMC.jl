@@ -364,6 +364,32 @@ function summary_finish(record::Array{Float64,3})
     rc == 0 || throw(ArgumentError("summary record"))
     (; mean, sd, mcse, ess, rhat, rank, draws)
 end
+"""`mcmc_summary` that also counts the kept draws into `nbins` bins of the grid `lo`, `hi` [D, P] plus a tail bin on each side
+(dhmc_mcmc_summary_histogram) and returns `(; record, counts, q, q_lo, q_hi)`: counts [nbins + 2, D, P] (shards on one grid
+add), and the bracketed quantiles [length(quantiles), D, P] of `histogram_quantiles`."""
+function mcmc_summary(h::Handle, N::Integer, P::Integer, lo::AbstractMatrix, hi::AbstractMatrix; quantiles,
+                      nbins::Integer = 256, thin::Integer = 1, reference = nothing)
+    record = Array{Float64}(undef, SUMMARY_FIELDS, h.D, P)
+    counts = zeros(Int64, nbins + 2, h.D, P)
+    lo, hi = convert(Matrix{Float64}, lo), convert(Matrix{Float64}, hi)
+    ref = reference === nothing ? C_NULL : convert(Matrix{Float64}, reference)
+    _ck(h, ccall((:dhmc_mcmc_summary_histogram, LIB), Cint,
+                 (Ptr{Cvoid}, Int32, Int32, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Int32, Ptr{Float64}, Ptr{Int64}, Ptr{Cvoid}, Ptr{Float64}),
+                 h.ptr, N, thin, ref, lo, hi, nbins, record, counts, C_NULL, C_NULL))
+    (; record, counts, histogram_quantiles(counts, lo, hi, quantiles)...)
+end
+"""q, q_lo, q_hi [length(probs), D, P] of counts [nbins + 2, D, P] on the grid lo, hi [D, P] (dhmc_histogram_quantiles):
+the exact type-7 quantile of the counted draws lies in [q_lo, q_hi]; q is NaN when it needs a tail bin."""
+function histogram_quantiles(counts::Array{Int64,3}, lo::Matrix{Float64}, hi::Matrix{Float64}, probs)
+    nb, D, P = size(counts, 1) - 2, size(counts, 2), size(counts, 3)
+    p = convert(Vector{Float64}, collect(probs))
+    q, q_lo, q_hi = (Array{Float64}(undef, length(p), D, P) for _ in 1:3)
+    rc = ccall((:dhmc_histogram_quantiles, LIB), Cint,
+               (Ptr{Int64}, Ptr{Float64}, Ptr{Float64}, Int32, Int64, Int64, Ptr{Float64}, Int32, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}),
+               counts, lo, hi, nb, D, P, p, length(p), q, q_lo, q_hi)
+    rc == 0 || throw(ArgumentError("histogram quantiles: probabilities in [0, 1] and a valid grid"))
+    (; q, q_lo, q_hi)
+end
 
 # ---- mcmc_steps / mcmc_next_step — src/mcmc.jl:335-351: stepwise sampling at the adapted (κ, ϵ) -----
 struct MCMCSteps; h::Handle; end
