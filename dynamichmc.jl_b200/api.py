@@ -227,6 +227,13 @@ class UserLogDensity(DeviceLogDensity):
     def params(self):
         return self._params
 
+    def generated_count(self):
+        """G: the generated quantities the header declares at this dimension (include/dhmc_models.h), 0 without them."""
+        G = C.c_int32()
+        _argcheck(L.lib(self.library_path).dhmc_user_generated_count(C.c_int64(self.D), C.byref(G)) == L.DHMC_OK,
+                  f"{self.library_path} carries no user model")
+        return G.value
+
     def model_name(self):
         buf = C.create_string_buffer(128)
         rc = L.lib(self.library_path).dhmc_user_family_name(buf, C.c_size_t(128))
@@ -419,6 +426,7 @@ class GaussianKineticEnergy:
 # ------------------------------------------------------------------ engine
 class Engine:
     """Owns a dhmc_handle: K chains of one problem (or of a ProblemBatch) on one GPU."""
+    _G = 0            # generated quantities of the handle's model (dhmc_generated_count, set per handle)
 
     def __init__(self, ℓ: DeviceLogDensity, chains: int, seed: int = 0, algorithm: NUTS = None,
                  device: int = 0, chain_offset: int = 0, threads_per_chain: int = 0,
@@ -439,6 +447,10 @@ class Engine:
                 raise ArgumentError(msg)
             raise RuntimeError(f"dhmc_create failed [{rc}]: {msg}")
         self._h = h
+        self.chain_offset = int(chain_offset)
+        G = C.c_int32()
+        self._ck(self._lib.dhmc_generated_count(h, C.byref(G)))
+        self._G = G.value
         self._set_problem(ℓ)
 
     def _set_problem(self, ℓ):
@@ -689,6 +701,55 @@ class Engine:
                                              L.ptr(stats), L.ptr(ld)))
         return dict(posterior_matrix=post, tree_statistics=stats, logdensities=ld)
 
+    @property
+    def generated_count(self):
+        """G: the generated quantities of the handle's model (a user model with DHMC_USER_GENERATED), 0 without them."""
+        return self._G
+
+    def _n_problems(self):
+        return self.ℓ.n_problems if isinstance(self.ℓ, ProblemBatch) else 1
+
+    def generated(self, theta, problem=None):
+        """The G generated quantities of positions `theta` (numpy; dhmc_generated, evaluated on the device) with the last
+        axis G in place of D.  Each point reads the parameter block of its problem:
+          [D]          one point of `problem` (default 0)
+          [n, D]       n points of `problem`; without one, of problem 0 on a one-problem handle, else one point per
+                       problem (n = P: per-problem references)
+          [K, N, D]    the posterior_matrix of mcmc: chain k's draws read the problem of global chain chain_offset + k,
+                       or all read `problem`"""
+        _argcheck(self._G > 0, "the model has no generated quantities (include/dhmc_models.h DHMC_USER_GENERATED)")
+        th = np.ascontiguousarray(theta, float)
+        _argcheck(th.ndim in (1, 2, 3) and th.shape[-1] == self.D, f"theta: [..., D] with D = {self.D}")
+        P, G = self._n_problems(), self._G
+        out = np.empty(th.shape[:-1] + (G,))
+        if problem is not None:
+            _argcheck(int(problem) == problem and 0 <= problem < P, f"problem: 0 … {P - 1}")
+            runs = [(int(problem), 0, th.size // self.D)]                     # (problem, first point, points)
+        elif th.ndim == 3:
+            _argcheck(th.shape[0] == self.K, f"theta [K, N, D]: the K = {self.K} chains of the handle, or name a problem")
+            kp = self.ℓ.chains_per_problem if isinstance(self.ℓ, ProblemBatch) else 0
+            prob = (self.chain_offset + np.arange(self.K)) // kp if kp else np.zeros(self.K, np.int64)
+            N = th.shape[1]
+            runs = []
+            for k in range(self.K):                                        # consecutive chains of one problem: one run
+                if runs and runs[-1][0] == prob[k]:
+                    runs[-1][2] += N
+                else:
+                    runs.append([int(prob[k]), k * N, N])
+            if len({r[2] for r in runs}) == 1 and len(runs) > 1:          # whole problems: one call over all of them
+                self._ck(self._lib.dhmc_generated(self._h, L.ptr(th), runs[0][2], runs[0][0], len(runs), L.ptr(out)))
+                return out
+        elif th.ndim == 2 and P > 1:
+            _argcheck(th.shape[0] == P, f"theta [n, D] without a problem: one point per problem (n = P = {P})")
+            self._ck(self._lib.dhmc_generated(self._h, L.ptr(th), 1, 0, P, L.ptr(out)))
+            return out
+        else:
+            runs = [(0, 0, th.size // self.D)]
+        flat, fout = th.reshape(-1, self.D), out.reshape(-1, G)
+        for p, first, n in runs:
+            self._ck(self._lib.dhmc_generated(self._h, L.ptr(flat[first:]), n, p, 1, L.ptr(fout[first:])))
+        return out
+
     def mcmc_summary(self, N, thin=1, reference=None, stats=False, quantiles=None, grid=None, bins=256):
         """N transitions as mcmc (same draws, same final state and transition count), every thin-th kept and folded on the
         device into per-(problem, parameter) statistics instead of being returned (dhmc_mcmc_summary, DESIGN §4.4).
@@ -703,15 +764,25 @@ class Engine:
         equal bins between lo and hi plus one tail bin on each side (dhmc_mcmc_summary_histogram) and adds `quantile`,
         `quantile_lo`, `quantile_hi` [P, D, len(quantiles)] (the exact quantile of the kept draws lies in [quantile_lo,
         quantile_hi]; diagnostics.histogram_quantiles), `histogram` [P, D, bins + 2] (exact counts: those of shards on one
-        grid add up), `grid` and `probs`."""
+        grid add up), `grid` and `probs`.
+
+        A model with G generated quantities (generated_count) is summarized on R = D + G rows: the D parameters, then the
+        G quantities of every kept draw.  Every [P, D] above is then [P, R]; a `reference` [P, D] is extended with its
+        generated quantities (Engine.generated), one [P, R] is taken as given."""
         from . import diagnostics
         _argcheck(N >= 1 and thin >= 1 and N % thin == 0, "N ≥ 1, thin ≥ 1 and N a multiple of thin")
         _argcheck(N // thin >= 4, "at least 4 kept draws per chain (N / thin ≥ 4)")
-        P = self.ℓ.n_problems if isinstance(self.ℓ, ProblemBatch) else 1
+        P = self._n_problems()
+        R = self.D + self._G
         ref = None
         if reference is not None:
             ref = np.ascontiguousarray(reference, float)
-            _argcheck(ref.shape == (P, self.D), f"reference: [P, D] = ({P}, {self.D})")
+            if self._G:
+                _argcheck(ref.shape in ((P, self.D), (P, R)), f"reference: [P, D] = ({P}, {self.D}) or [P, D + G] = ({P}, {R})")
+                if ref.shape == (P, self.D):
+                    ref = np.ascontiguousarray(np.concatenate([ref, self.generated(ref)], axis=1))
+            else:
+                _argcheck(ref.shape == (P, self.D), f"reference: [P, D] = ({P}, {self.D})")
         _argcheck(quantiles is not None or grid is None, "grid without quantiles")
         counts = None
         if quantiles is not None:
@@ -719,10 +790,10 @@ class Engine:
             _argcheck(probs.ndim == 1 and probs.size >= 1 and np.all((probs >= 0.0) & (probs <= 1.0)),
                       "quantiles: probabilities in [0, 1]")
             _argcheck(grid is not None and len(grid) == 2, "quantiles need grid = (lo, hi), each [P, D]")
-            lo, hi = diagnostics.check_grid(grid[0], grid[1], bins, (P, self.D))
+            lo, hi = diagnostics.check_grid(grid[0], grid[1], bins, (P, R))
             bins = int(bins)
-            counts = np.zeros((P, self.D, bins + 2), np.int64)
-        record = np.zeros((P, self.D, L.SUMMARY_FIELDS))
+            counts = np.zeros((P, R, bins + 2), np.int64)
+        record = np.zeros((P, R, L.SUMMARY_FIELDS))
         n = N // thin
         st = np.zeros((self.K, n), dtype=L.tree_stats_dtype) if stats else None
         ld = np.empty((self.K, n)) if stats else None
@@ -736,9 +807,9 @@ class Engine:
         out = self.summary_finish(record)
         out["record"] = record
         if counts is not None:
-            shape = (P, self.D, probs.size)
+            shape = (P, R, probs.size)
             q, q_lo, q_hi = np.empty(shape), np.empty(shape), np.empty(shape)
-            self._ck(self._lib.dhmc_histogram_quantiles(L.ptr(counts), L.ptr(lo), L.ptr(hi), bins, self.D, P, L.ptr(probs),
+            self._ck(self._lib.dhmc_histogram_quantiles(L.ptr(counts), L.ptr(lo), L.ptr(hi), bins, R, P, L.ptr(probs),
                                                         probs.size, L.ptr(q), L.ptr(q_lo), L.ptr(q_hi)))
             out.update(quantile=q, quantile_lo=q_lo, quantile_hi=q_hi, histogram=counts, grid=(lo, hi), probs=probs)
         if stats:

@@ -51,6 +51,10 @@ const void* dhmc_user_family_kernel_0(int W, int epl, int kernel, int dense) DHM
 const void* dhmc_user_family_kernel_3(int W, int epl, int kernel, int dense) DHMC_TU_LINKAGE;
 const char* dhmc_user_family_name_str(void) DHMC_TU_LINKAGE;
 int dhmc_user_family_min_dim(void) DHMC_TU_LINKAGE;
+// generated quantities (a model with DHMC_USER_GENERATED): G(D) and the launch of k_generated (family_tu.cu)
+int dhmc_user_family_ngq(int D) DHMC_TU_LINKAGE;
+int dhmc_user_family_generated(const double* theta, long long n, long long n_problems, int D, int ng, const double* mparams,
+                               const void* problems, long long first, double* out, int T, int grid, cudaStream_t stream) DHMC_TU_LINKAGE;
 }
 // part: 0 = one chain per CTA, 1 = packed chain groups (likelihood on the tensor cores),
 // 3 = one chain per CTA with max_depth > 12 (persistent kernels only)
@@ -363,6 +367,7 @@ struct dhmc_handle {
   void* sum_buf = nullptr;
   size_t sum_bytes = 0;
   SummaryArgs* sum_args = nullptr;
+  int ngq = 0;                      // generated quantities of a user model (dhmc_generated_count)
   std::string err;
 };
 
@@ -645,6 +650,11 @@ int dhmc_create(const dhmc_config* cfg, dhmc_handle** out) {
     pack = kPack;
   }
   if (T == 0 || EPL == 0) { g_create_err = "dim too large for this build (dim <= 32 * threads_per_chain, 32 only for 256 threads: dim <= 8192)"; return DHMC_EARG; }
+  const int ngq = cfg->family == DHMC_FAMILY_USER && dhmc_user_family_ngq ? dhmc_user_family_ngq((int)cfg->dim) : 0;
+  if (cfg->family == DHMC_FAMILY_USER && dhmc_user_family_ngq && !(ngq >= 1 && ngq <= DHMC_MAX_GENERATED)) {
+    g_create_err = "the user model's dhmc_user_ngq(dim) is outside [1, 8192]";
+    return DHMC_EARG;
+  }
   int ndev = 0;
   cudaError_t ce = cudaGetDeviceCount(&ndev);
   if (ce != cudaSuccess || ndev == 0) {
@@ -655,6 +665,7 @@ int dhmc_create(const dhmc_config* cfg, dhmc_handle** out) {
   if (cfg->device < 0 || cfg->device >= ndev) { g_create_err = "bad device ordinal"; return DHMC_EARG; }
   dhmc_handle* h = new dhmc_handle();
   h->cfg = *cfg; h->T = T; h->W = T / 32; h->EPL = EPL; h->stride = (size_t)T * EPL; h->G = pack; h->deep = deep;
+  h->ngq = ngq;
   h->n_slots = slots_needed(cfg->max_depth);
   h->levels = deep ? cfg->max_depth + 1 : kStdLevels;        // deep persistent kernels size their stack / slot table at run time
   h->ntab = deep ? std::max(kStdTab, (h->n_slots + 7) & ~7) : kStdTab;
@@ -1398,6 +1409,78 @@ static bool valid_grid(const double* lo, const double* hi, int nbins, size_t cel
   return true;
 }
 
+// rows [r0, r0 + n) of every problem of a host array [P][R] into the device array [P][n]
+static cudaError_t upload_rows(double* dst, const double* src, size_t r0, size_t n, size_t R, size_t P, cudaStream_t s) {
+  if (n == R) return cudaMemcpyAsync(dst, src, sizeof(double) * P * R, cudaMemcpyHostToDevice, s);
+  return cudaMemcpy2DAsync(dst, sizeof(double) * n, src + r0, sizeof(double) * R, sizeof(double) * n, P, cudaMemcpyHostToDevice, s);
+}
+
+// generated quantities of device points theta [n_problems][n][D] (problem first + j owns points j·n … (j+1)·n − 1) into
+// out [n_problems][n][G] on the handle's stream (k_generated, family_tu.cu); the caller has checked the arguments
+static int launch_generated(dhmc_handle* h, const double* theta, int64_t n, int64_t first, int64_t n_problems, double* out) {
+  const int64_t pts = n * n_problems;
+  const int grid = (int)std::min<int64_t>(pts, (int64_t)h->sm_count * 16);
+  const int e = dhmc_user_family_generated(theta, n, n_problems, (int)h->cfg.dim, h->ngq, h->mparams,
+                                           h->batch_k ? h->problems : nullptr, first, out, h->T, grid, h->stream);
+  if (e != cudaSuccess) { h->err = std::string("k_generated: ") + cudaGetErrorString((cudaError_t)e); return DHMC_ECUDA; }
+  h->launches += 1;
+  return DHMC_OK;
+}
+
+// dhmc_generated(_dev): DHMC_EARG before anything runs for a handle without generated quantities, NULL pointers, n < 1,
+// n_problems < 1 or a problem range outside the handle's batch
+static int check_generated(dhmc_handle* h, const double* theta, int64_t n, int64_t first, int64_t n_problems, const double* out) {
+  const int64_t P = h->batch_k ? h->batch_p : 1;
+  if (h->ngq == 0) { h->err = "dhmc_generated: the handle's model has no generated quantities"; return DHMC_EARG; }
+  if (!theta || !out) { h->err = "dhmc_generated: theta or out is NULL"; return DHMC_EARG; }
+  if (n < 1 || n_problems < 1 || first < 0 || first > P - n_problems) {
+    h->err = "dhmc_generated: n ≥ 1, and problems first … first + n_problems − 1 of the handle's batch";
+    return DHMC_EARG;
+  }
+  return DHMC_OK;
+}
+
+int dhmc_user_generated_count(int64_t dim, int32_t* G) {
+  if (!dhmc_user_family_name_str || !G || dim < 1 || dim > INT32_MAX) return DHMC_EARG;
+  *G = dhmc_user_family_ngq ? dhmc_user_family_ngq((int)dim) : 0;
+  return DHMC_OK;
+}
+
+int dhmc_generated_count(dhmc_handle* h, int32_t* G) {
+  if (!h || !G) return DHMC_EARG;
+  *G = h->ngq;
+  return DHMC_OK;
+}
+
+int dhmc_generated_dev(dhmc_handle* h, const double* theta, int64_t n, int64_t first_problem, int64_t n_problems, double* out) {
+  if (!h) return DHMC_EARG;
+  const int rc = check_generated(h, theta, n, first_problem, n_problems, out);
+  if (rc != DHMC_OK) return rc;
+  CK(cudaSetDevice(h->cfg.device));
+  const int rg = launch_generated(h, theta, n, first_problem, n_problems, out);
+  if (rg != DHMC_OK) return rg;
+  CK(cudaStreamSynchronize(h->stream));
+  return DHMC_OK;
+}
+
+int dhmc_generated(dhmc_handle* h, const double* theta, int64_t n, int64_t first_problem, int64_t n_problems, double* out) {
+  if (!h) return DHMC_EARG;
+  const int rc = check_generated(h, theta, n, first_problem, n_problems, out);
+  if (rc != DHMC_OK) return rc;
+  CK(cudaSetDevice(h->cfg.device));
+  const size_t pts = (size_t)n * (size_t)n_problems, D = (size_t)h->cfg.dim, G = (size_t)h->ngq;
+  double* buf = nullptr;
+  CK(cudaMalloc(&buf, sizeof(double) * pts * (D + G)));
+  cudaError_t e = cudaMemcpyAsync(buf, theta, sizeof(double) * pts * D, cudaMemcpyHostToDevice, h->stream);
+  int rg = e == cudaSuccess ? launch_generated(h, buf, n, first_problem, n_problems, buf + pts * D) : DHMC_OK;
+  if (e == cudaSuccess && rg == DHMC_OK)
+    e = cudaMemcpyAsync(out, buf + pts * D, sizeof(double) * pts * G, cudaMemcpyDeviceToHost, h->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+  cudaFree(buf);
+  if (e != cudaSuccess) { h->err = std::string("dhmc_generated: ") + cudaGetErrorString(e); return DHMC_ECUDA; }
+  return rg;
+}
+
 // dhmc_mcmc_summary and, with counts, dhmc_mcmc_summary_histogram (arguments checked by the caller)
 static int mcmc_summary(dhmc_handle* h, int32_t N, int32_t thin, const double* reference, const double* lo_host,
                         const double* hi_host, int32_t nbins, double* record, int64_t* counts, dhmc_tree_stats* stats,
@@ -1413,9 +1496,15 @@ static int mcmc_summary(dhmc_handle* h, int32_t N, int32_t thin, const double* r
   const size_t P = K ? (size_t)h->batch_p : 1, PD = P * D, rows = (size_t)h->grid * h->G * 3 * D;
   // histograms (counts != NULL): cells bins per (d, p); the staging rows of the resident chain groups
   const size_t cells = counts ? (size_t)nbins + 2 : 0, stage = (size_t)h->grid * h->G * cells * D;
+  // generated quantities: ng rows after the D parameter rows of every host array (R = D + ng rows), and on the device the
+  // arrays of SummaryArgs' g-fields, laid out as the parameters' with ng in place of D
+  const size_t ng = (size_t)h->ngq, R = D + ng, PG = P * ng, grows = (size_t)h->grid * h->G * 5 * ng;
+  const size_t gstage = (size_t)h->grid * h->G * cells * ng;
   // one grow-only arena: acc [P][5][D], shift [P][D], ref [P][D], row [grid·G][3][D], below [P][D], chains [P], then with
-  // histograms hist [P][D][cells], lo [P][D], inv_w [P][D] (8-byte elements) and stage [grid·G][cells][D] (4-byte)
-  const size_t need = sizeof(double) * (8 * PD + rows + P + PD * cells + (counts ? 2 * PD : 0)) + sizeof(unsigned) * stage;
+  // histograms hist [P][D][cells], lo [P][D], inv_w [P][D]; the same for the generated quantities (gacc, gshift, gref, grow,
+  // gbelow, ghist, glo, ginv_w; 8-byte elements); last stage [grid·G][cells][D] and gstage [grid·G][cells][ng] (4-byte)
+  const size_t need = sizeof(double) * (8 * PD + rows + P + PD * cells + (counts ? 2 * PD : 0)) + sizeof(unsigned) * stage +
+                      sizeof(double) * (8 * PG + grows + PG * cells + (counts ? 2 * PG : 0)) + sizeof(unsigned) * gstage;
   if (need > h->sum_bytes) {
     cudaFree(h->sum_buf); h->sum_buf = nullptr; h->sum_bytes = 0;
     CK(cudaMalloc(&h->sum_buf, need));
@@ -1430,7 +1519,7 @@ static int mcmc_summary(dhmc_handle* h, int32_t N, int32_t thin, const double* r
   unsigned long long* chains = below + PD;
   CK(cudaMemsetAsync(acc, 0, sizeof(double) * 5 * PD, h->stream));
   CK(cudaMemsetAsync(below, 0, sizeof(unsigned long long) * (PD + P), h->stream));
-  if (reference) CK(cudaMemcpyAsync(ref, reference, sizeof(double) * PD, cudaMemcpyHostToDevice, h->stream));
+  if (reference) CK(upload_rows(ref, reference, 0, D, R, P, h->stream));
   // shift of problem p: the position of its first local chain, max(p·K − off, 0); problems p0 … p1 have local chains.  Past
   // the first, those chains are K apart: one strided copy (a first problem entered in its middle takes one more).
   const int64_t p0 = K ? off / K : 0, p1 = K ? (off + (int64_t)B - 1) / K : 0;
@@ -1440,48 +1529,85 @@ static int mcmc_summary(dhmc_handle* h, int32_t N, int32_t thin, const double* r
     CK(cudaMemcpy2DAsync(shift + pa * D, sizeof(double) * D, h->q + (size_t)(K ? pa * K - off : 0) * D, sizeof(double) * D * (size_t)(K ? K : 1),
                          sizeof(double) * D, (size_t)(p1 - pa + 1), cudaMemcpyDeviceToDevice, h->stream));
   SummaryArgs sa{row, shift, reference ? ref : nullptr, acc, below, chains, n_keep / 2, nullptr, nullptr, nullptr, nullptr, 0};
+  unsigned long long* hist = chains + P;
+  double* lo = (double*)(hist + PD * cells);
+  double* inv_w = lo + PD;
+  double* gacc = counts ? inv_w + PD : (double*)hist;
+  std::vector<double> hinv(counts ? P * R : 0);
+  for (size_t i = 0; i < hinv.size(); ++i) hinv[i] = (double)nbins / (hi_host[i] - lo_host[i]);
   if (counts) {
-    unsigned long long* hist = chains + P;
-    double* lo = (double*)(hist + PD * cells);
-    double* inv_w = lo + PD;
-    std::vector<double> hinv(PD);
-    for (size_t i = 0; i < PD; ++i) hinv[i] = (double)nbins / (hi_host[i] - lo_host[i]);
     CK(cudaMemsetAsync(hist, 0, sizeof(unsigned long long) * PD * cells, h->stream));
-    CK(cudaMemcpyAsync(lo, lo_host, sizeof(double) * PD, cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemcpyAsync(inv_w, hinv.data(), sizeof(double) * PD, cudaMemcpyHostToDevice, h->stream));
-    sa.lo = lo; sa.inv_w = inv_w; sa.stage = (unsigned*)(inv_w + PD); sa.hist = hist; sa.nbins = nbins;
+    CK(upload_rows(lo, lo_host, 0, D, R, P, h->stream));
+    CK(upload_rows(inv_w, hinv.data(), 0, D, R, P, h->stream));
+    sa.lo = lo; sa.inv_w = inv_w; sa.stage = (unsigned*)(gacc + 8 * PG + grows + PG * cells + 2 * PG); sa.hist = hist; sa.nbins = nbins;
+  }
+  // generated quantities: gacc [P][5][ng], gshift, gref [P][ng], grow [grid·G][5][ng], gbelow [P][ng], then with histograms
+  // ghist [P][ng][cells], glo, ginv_w [P][ng]; the shift is g(shift), evaluated on the device
+  double* gshift = gacc + 5 * PG;
+  double* gref = gshift + PG;
+  double* grow = gref + PG;
+  unsigned long long* gbelow = (unsigned long long*)(grow + grows);
+  unsigned long long* ghist = gbelow + PG;
+  if (ng) {
+    CK(cudaMemsetAsync(gacc, 0, sizeof(double) * 5 * PG, h->stream));
+    CK(cudaMemsetAsync(gbelow, 0, sizeof(unsigned long long) * PG, h->stream));
+    const int rg = launch_generated(h, shift + p0 * D, 1, p0, p1 - p0 + 1, gshift + p0 * ng);
+    if (rg != DHMC_OK) return rg;
+    if (reference) CK(upload_rows(gref, reference, D, ng, R, P, h->stream));
+    sa.ng = (int)ng; sa.mparams = h->mparams; sa.problems = K ? h->problems : nullptr;
+    sa.grow = grow; sa.gshift = gshift; sa.gref = reference ? gref : nullptr; sa.gacc = gacc; sa.gbelow = gbelow;
+    if (counts) {
+      double* glo = (double*)(ghist + PG * cells);
+      double* ginv_w = glo + PG;
+      CK(cudaMemsetAsync(ghist, 0, sizeof(unsigned long long) * PG * cells, h->stream));
+      CK(upload_rows(glo, lo_host, D, ng, R, P, h->stream));
+      CK(upload_rows(ginv_w, hinv.data(), D, ng, R, P, h->stream));
+      sa.glo = glo; sa.ginv_w = ginv_w; sa.gstage = sa.stage + stage; sa.ghist = ghist;
+    }
   }
   CK(cudaMemcpyAsync(h->sum_args, &sa, sizeof sa, cudaMemcpyHostToDevice, h->stream));
   AdaptConfig cfg{};
   const int rc = run_nuts(h, N, cfg, 0.0, nullptr, nullptr, nullptr, stats, nullptr, logdens, false, true, nullptr, thin, false,
                           h->sum_args);
   if (rc != DHMC_OK && rc != DHMC_ENUMERIC) return rc;    // a chain that failed is left out of its problem's sums
-  std::vector<double> hacc(5 * PD), hshift(PD);
-  std::vector<unsigned long long> hcnt(PD + P);
+  std::vector<double> hacc(5 * PD), hshift(PD), hgacc(5 * PG), hgshift(PG);
+  std::vector<unsigned long long> hcnt(PD + P), hgcnt(PG);
   CK(cudaMemcpyAsync(hacc.data(), acc, sizeof(double) * hacc.size(), cudaMemcpyDeviceToHost, h->stream));
   CK(cudaMemcpyAsync(hshift.data(), shift, sizeof(double) * PD, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaMemcpyAsync(hcnt.data(), below, sizeof(unsigned long long) * hcnt.size(), cudaMemcpyDeviceToHost, h->stream));
-  if (counts)        // [P][D][cells] is the column-major [cells, D, P] of the ABI; uint64 counts stay far below 2^63
-    CK(cudaMemcpyAsync(counts, below + PD + P, sizeof(int64_t) * PD * cells, cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  for (size_t p = 0; p < P; ++p) {
-    const double M = (double)hcnt[PD + p], m = 2.0 * M;
-    const double* a = &hacc[p * 5 * D];
-    for (size_t d = 0; d < D; ++d) {
-      double* r = summary_cell(record, (int64_t)D, (int64_t)p, (int64_t)d);
-      r[DHMC_SUMMARY_CHAINS] = M;
-      r[DHMC_SUMMARY_NKEEP] = (double)n_keep;
-      r[DHMC_SUMMARY_BELOW] = reference ? (double)hcnt[p * D + d] : dm_nan();
-      if (M == 0) {
-        r[DHMC_SUMMARY_MEAN] = r[DHMC_SUMMARY_SS_SEQ] = r[DHMC_SUMMARY_M2] = r[DHMC_SUMMARY_SS_CHAIN] = 0.0;
-        continue;
-      }
-      const double s1 = a[d], s2 = a[D + d], c1 = a[3 * D + d], c2 = a[4 * D + d];
-      r[DHMC_SUMMARY_MEAN] = hshift[p * D + d] + s1 / m;
-      r[DHMC_SUMMARY_SS_SEQ] = std::max(0.0, s2 - s1 * s1 / m);
-      r[DHMC_SUMMARY_M2] = a[2 * D + d];
-      r[DHMC_SUMMARY_SS_CHAIN] = std::max(0.0, c2 - c1 * c1 / M);
+  // [P][D][cells] is the column-major [cells, D, P] of the ABI; uint64 counts stay far below 2^63
+  if (counts && !ng) CK(cudaMemcpyAsync(counts, below + PD + P, sizeof(int64_t) * PD * cells, cudaMemcpyDeviceToHost, h->stream));
+  if (ng) {            // counts [cells, R, P]: the D parameter rows, then the ng generated rows of each problem
+    CK(cudaMemcpyAsync(hgacc.data(), gacc, sizeof(double) * hgacc.size(), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(hgshift.data(), gshift, sizeof(double) * PG, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(hgcnt.data(), gbelow, sizeof(unsigned long long) * PG, cudaMemcpyDeviceToHost, h->stream));
+    if (counts) {
+      const size_t c8 = sizeof(int64_t) * cells;
+      CK(cudaMemcpy2DAsync(counts, c8 * R, hist, c8 * D, c8 * D, P, cudaMemcpyDeviceToHost, h->stream));
+      CK(cudaMemcpy2DAsync(counts + D * cells, c8 * R, ghist, c8 * ng, c8 * ng, P, cudaMemcpyDeviceToHost, h->stream));
     }
+  }
+  CK(cudaStreamSynchronize(h->stream));
+  // row d of problem p from its sums a[·], its shift and its below-count (the sums of n rows, [5][n])
+  auto finish = [&](size_t p, size_t r_out, const double* a, size_t n, size_t d, double sh, unsigned long long nb) {
+    const double M = (double)hcnt[PD + p], m = 2.0 * M;
+    double* r = summary_cell(record, (int64_t)R, (int64_t)p, (int64_t)r_out);
+    r[DHMC_SUMMARY_CHAINS] = M;
+    r[DHMC_SUMMARY_NKEEP] = (double)n_keep;
+    r[DHMC_SUMMARY_BELOW] = reference ? (double)nb : dm_nan();
+    if (M == 0) {
+      r[DHMC_SUMMARY_MEAN] = r[DHMC_SUMMARY_SS_SEQ] = r[DHMC_SUMMARY_M2] = r[DHMC_SUMMARY_SS_CHAIN] = 0.0;
+      return;
+    }
+    const double s1 = a[d], s2 = a[n + d], c1 = a[3 * n + d], c2 = a[4 * n + d];
+    r[DHMC_SUMMARY_MEAN] = sh + s1 / m;
+    r[DHMC_SUMMARY_SS_SEQ] = std::max(0.0, s2 - s1 * s1 / m);
+    r[DHMC_SUMMARY_M2] = a[2 * n + d];
+    r[DHMC_SUMMARY_SS_CHAIN] = std::max(0.0, c2 - c1 * c1 / M);
+  };
+  for (size_t p = 0; p < P; ++p) {
+    for (size_t d = 0; d < D; ++d) finish(p, d, &hacc[p * 5 * D], D, d, hshift[p * D + d], hcnt[p * D + d]);
+    for (size_t k = 0; k < ng; ++k) finish(p, D + k, &hgacc[p * 5 * ng], ng, k, hgshift[p * ng + k], hgcnt[p * ng + k]);
   }
   return rc;
 }
@@ -1497,7 +1623,7 @@ int dhmc_mcmc_summary_histogram(dhmc_handle* h, int32_t N, int32_t thin, const d
                                 double* logdens) {
   if (!h) return DHMC_EARG;
   if (!counts) { h->err = "dhmc_mcmc_summary_histogram: counts is NULL"; return DHMC_EARG; }
-  const size_t cells = (size_t)h->cfg.dim * (h->batch_k ? (size_t)h->batch_p : 1);
+  const size_t cells = ((size_t)h->cfg.dim + (size_t)h->ngq) * (h->batch_k ? (size_t)h->batch_p : 1);
   if (!valid_grid(lo, hi, nbins, cells)) {
     h->err = "dhmc_mcmc_summary_histogram: 1 ≤ nbins ≤ 4096 and, per cell, finite lo < hi with hi − lo and nbins / (hi − lo) finite";
     return DHMC_EARG;

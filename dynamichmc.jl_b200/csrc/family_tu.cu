@@ -26,6 +26,29 @@ extern "C" __attribute__((visibility("hidden"))) const void* dhmc_user_family_ke
 }
 extern "C" __attribute__((visibility("hidden"))) const char* dhmc_user_family_name_str(void) { return DHMC_USER_NAME; }
 extern "C" __attribute__((visibility("hidden"))) int dhmc_user_family_min_dim(void) { return DHMC_USER_MIN_DIM; }
+#ifdef DHMC_USER_GENERATED
+// Generated quantities at given points (dhmc_generated): one CTA of T threads (the handle's chain width) per point, thread
+// tid writing quantities k = tid + e·T.  theta [n_problems][n][D], out [n_problems][n][G]; the points of local problem j
+// read the parameter block of problem first + j (problems null: the handle's one problem).
+namespace dhmc {
+__global__ void k_generated(const double* theta, long long n, long long n_problems, int D, int ng, const double* mparams,
+                            const ProblemDesc* problems, long long first, double* out) {
+  for (long long pt = blockIdx.x; pt < n * n_problems; pt += gridDim.x) {
+    const double* params = mparams + (problems ? problems[first + pt / n].mparams : 0);
+    const double* q = theta + (size_t)pt * D;
+    for (int k = threadIdx.x; k < ng; k += blockDim.x) out[(size_t)pt * ng + k] = dhmc_user_generated(k, D, q, params);
+  }
+}
+}  // namespace dhmc
+extern "C" __attribute__((visibility("hidden"))) int dhmc_user_family_ngq(int D) { return dhmc_user_ngq(D); }
+extern "C" __attribute__((visibility("hidden"))) int dhmc_user_family_generated(const double* theta, long long n, long long n_problems,
+                                                                                int D, int ng, const double* mparams, const void* problems,
+                                                                                long long first, double* out, int T, int grid,
+                                                                                cudaStream_t stream) {
+  dhmc::k_generated<<<grid, T, 0, stream>>>(theta, n, n_problems, D, ng, mparams, (const dhmc::ProblemDesc*)problems, first, out);
+  return (int)cudaGetLastError();
+}
+#endif
 #elif DHMC_TU_PART == 3
 extern "C" __attribute__((visibility("hidden"))) const void* dhmc_user_family_kernel_3(int W, int epl, int kernel, int dense) {
   return dhmc::family_kernel_ptr<DHMC_FAMILY_USER, 3>(W, epl, (dhmc::KernelId)kernel, dense != 0);

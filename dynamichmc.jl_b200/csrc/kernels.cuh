@@ -43,6 +43,11 @@ struct ProblemDesc {
 //   lo, inv_w [P][D]                 the grid: lower end and nbins / (hi − lo)
 //   stage [grid·G][nbins + 2][D]     per chain group: the counts of the running chain (cleared at its first kept draw)
 //   hist  [P][D][nbins + 2]          Σ over the problem's completed chains (the host layout)
+// Generated quantities of a user model (include/dhmc_models.h; ng = 0: none), the summary's rows D … D + ng − 1, in arrays
+// of their own laid out as those of the parameters with ng in place of D (the parameters' arrays keep their layout):
+//   grow   [grid·G][5][ng]  per chain group: the running sequence's mean and M2, sequence 0's mean and M2, the below-count
+//   gshift, gref, gbelow, glo, ginv_w [P][ng];  gacc [P][5][ng];  gstage [grid·G][nbins + 2][ng];  ghist [P][ng][nbins + 2]
+//   mparams, problems   the problem blocks the quantities read (problems null: one problem)
 struct SummaryArgs {
   double* row;
   const double* shift;
@@ -56,6 +61,18 @@ struct SummaryArgs {
   unsigned* stage;
   unsigned long long* hist;
   int nbins;
+  int ng;
+  const double* mparams;
+  const ProblemDesc* problems;
+  double* grow;
+  const double* gshift;
+  const double* gref;
+  double* gacc;
+  unsigned long long* gbelow;
+  const double* glo;
+  const double* ginv_w;
+  unsigned* gstage;
+  unsigned long long* ghist;
 };
 
 struct KArgs {
@@ -359,6 +376,81 @@ __device__ __noinline__ void summary_hist_fold(const SummaryArgs* sp, int tid, i
     }
   }
 }
+#ifdef DHMC_USER_GENERATED
+// Generated quantities (include/dhmc_models.h), compiled only into a user library whose model declares them, so that every
+// other build keeps its code.  Quantity k reads the whole kept position, elements other threads wrote, so the chain
+// synchronises before it reads the slot and again before the next transition may overwrite it (one chain per CTA: the
+// USER family has no packed groups).  Thread tid evaluates and folds k = tid + e·T, with the moments, the rank and the bin
+// rule of the parameters; its state for k lives in grow, and nothing else reads it.
+template <class Bk>
+__device__ __noinline__ void summary_gq_draw(const SummaryArgs* sp, const double* zq, int tid, int grp, int D, size_t p, int j) {
+  static_assert(Bk::G == 1, "generated quantities: one chain per CTA");
+  constexpr int T = Bk::T;
+  const SummaryArgs& s = *sp;
+  const int ng = s.ng, n = s.n, nb = s.nbins;
+  const double* params = s.mparams + (s.problems ? s.problems[p].mparams : 0);
+  double* gr = s.grow + summary_group<Bk>(grp) * 5 * (size_t)ng;
+  unsigned* stage = s.ghist ? s.gstage + summary_group<Bk>(grp) * (size_t)(nb + 2) * (size_t)ng : nullptr;
+  __syncthreads();
+#pragma unroll 1
+  for (int k = tid; k < ng; k += T) {
+    const double v = dhmc_user_generated(k, D, zq, params);
+    if (j < 2 * n) {
+      const int kk = j < n ? j + 1 : j - n + 1;        // place in its sequence (1-based); metric_reset / metric_push
+      const double mean = kk == 1 ? 0.0 : gr[k], m2 = kk == 1 ? 0.0 : gr[ng + k];
+      const double dlt = v - mean;
+      const double mean1 = mean + dlt / (double)kk;
+      const double m21 = m2 + dlt * (v - mean1);
+      gr[k] = mean1; gr[ng + k] = m21;
+      if (j == n - 1) { gr[2 * ng + k] = mean1; gr[3 * ng + k] = m21; }
+    }
+    if (s.gref) {
+      const double below = v < s.gref[p * ng + k] ? 1.0 : 0.0;
+      gr[4 * ng + k] = j == 0 ? below : gr[4 * ng + k] + below;
+    }
+    if (stage) {
+      if (j == 0) {
+#pragma unroll 1
+        for (int c = 0; c < nb + 2; ++c) stage[(size_t)c * ng + k] = 0u;
+      }
+      const double t = __dmul_rn(__dsub_rn(v, s.glo[p * ng + k]), s.ginv_w[p * ng + k]);
+      const int c = t < 0.0 ? 0 : !(t < (double)nb) ? nb + 1 : 1 + (int)t;
+      stage[(size_t)c * ng + k] += 1u;
+    }
+  }
+  __syncthreads();
+}
+// chain end (completed chains only), as summary_fold
+template <class Bk>
+__device__ __noinline__ void summary_gq_fold(const SummaryArgs* sp, int tid, int grp, size_t p) {
+  constexpr int T = Bk::T;
+  const SummaryArgs& s = *sp;
+  const int ng = s.ng;
+  const size_t cells = (size_t)s.nbins + 2;
+  const double* gr = s.grow + summary_group<Bk>(grp) * 5 * (size_t)ng;
+  const unsigned* stage = s.ghist ? s.gstage + summary_group<Bk>(grp) * cells * (size_t)ng : nullptr;
+  double* acc = s.gacc + p * 5 * (size_t)ng;
+#pragma unroll 1
+  for (int k = tid; k < ng; k += T) {
+    const double sh = s.gshift[p * ng + k];
+    const double d0 = gr[2 * ng + k] - sh, d1 = gr[k] - sh, dc = 0.5 * (d0 + d1);
+    atomicAdd(acc + k, d0 + d1);
+    atomicAdd(acc + ng + k, d0 * d0 + d1 * d1);
+    atomicAdd(acc + 2 * ng + k, gr[3 * ng + k] + gr[ng + k]);
+    atomicAdd(acc + 3 * ng + k, dc);
+    atomicAdd(acc + 4 * ng + k, dc * dc);
+    if (s.gref) atomicAdd(s.gbelow + p * ng + k, (unsigned long long)gr[4 * ng + k]);
+    if (stage) {
+      unsigned long long* hist = s.ghist + (p * ng + k) * cells;
+#pragma unroll 1
+      for (size_t c = 0; c < cells; ++c) {
+        const unsigned cnt = stage[c * ng + k];
+        if (cnt) atomicAdd(hist + c, (unsigned long long)cnt);
+      }
+    }
+  }
+}
+#endif
 // kept draw j: sequence 0 is draws [0, n), sequence 1 draws [n, 2n); an odd last draw counts for the rank only
 template <class Bk>
 __device__ __noinline__ void summary_draw(const SummaryArgs* sp, double** slot_tab, int n_slots, int s_zq, int tid, int grp, int D,
@@ -396,6 +488,9 @@ __device__ __noinline__ void summary_draw(const SummaryArgs* sp, double** slot_t
     }
   }
   if (s.hist) summary_hist_draw<Bk>(sp, slot_tab[s_zq] + tid, tid, grp, D, p, j);
+#ifdef DHMC_USER_GENERATED
+  if (s.ng) summary_gq_draw<Bk>(sp, slot_tab[s_zq], tid, grp, D, p, j);
+#endif
 }
 // chain end (the chain completed the call): fold its two sequences into its problem's sums
 template <class Bk>
@@ -422,6 +517,9 @@ __device__ __noinline__ void summary_fold(const SummaryArgs* sp, double** slot_t
     }
   }
   if (s.hist) summary_hist_fold<Bk>(sp, tid, grp, Di, p);
+#ifdef DHMC_USER_GENERATED
+  if (s.ng) summary_gq_fold<Bk>(sp, tid, grp, p);
+#endif
   if (tid == 0) atomicAdd(s.chains + p, 1ull);
 }
 

@@ -138,6 +138,23 @@ int dhmc_user_family_name(char* name, size_t cap);
 /* Whether this library carries the kernels of `family` (the stock library: the four shipped families; a user-model
  * library: DHMC_FAMILY_USER only).  dhmc_create refuses an absent family with DHMC_EARG. */
 int dhmc_family_available(int32_t family, int32_t* available);
+/* Generated quantities (include/dhmc_models.h): G = dhmc_user_ngq(dim) functions of a position that a user model may
+ * declare (DHMC_USER_GENERATED), e.g. the centred effects of a non-centred model.  dhmc_create refuses a model whose
+ * G(dim) lies outside [1, DHMC_MAX_GENERATED].  They never affect sampling.  dhmc_generated_count gives G, 0 for the
+ * shipped families and for user models without them. */
+#define DHMC_MAX_GENERATED 8192
+int dhmc_generated_count(dhmc_handle* h, int32_t* G);
+/* The same G for dimension dim without a handle (no device needed): DHMC_EARG in a library without a user model. */
+int dhmc_user_generated_count(int64_t dim, int32_t* G);
+/* The G quantities of n·n_problems points: theta [D, n, n_problems] and out [G, n, n_problems], column-major; problem
+ * first_problem + j of the handle's batch (a handle without a batch is one problem) owns points j·n … (j+1)·n − 1 and
+ * lends them its parameter block.  So the draws [D, N, B] of a handle that holds whole problems are an input as they are
+ * (n = N·chains per problem), and so are per-problem references [D, P] (n = 1).  Evaluated on the device, one chain width
+ * of threads per point.  DHMC_EARG before anything runs for G = 0, NULL pointers, n < 1, n_problems < 1 or a problem
+ * range outside the batch.  dhmc_generated takes host arrays, dhmc_generated_dev device arrays. */
+int dhmc_generated(dhmc_handle* h, const double* theta, int64_t n, int64_t first_problem, int64_t n_problems, double* out);
+int dhmc_generated_dev(dhmc_handle* h, const double* theta, int64_t n, int64_t first_problem, int64_t n_problems,
+                       double* out);
 
 /* ---- state: initialization = (q, κ, ϵ), mcmc.jl:111-132 ---------------- */
 /* q: [D,B]; evaluates ℓ, ∇ℓ strictly (initialize_warmup_state, mcmc.jl:129-132). */
@@ -233,6 +250,12 @@ int dhmc_mcmc_dev(dhmc_handle* h, int32_t N, double* posterior, dhmc_tree_stats*
  *   draws  n_keep·M, the rank's denominator
  * A problem with no local chain gets NaN everywhere (rank 0, draws 0).  Quantiles: dhmc_mcmc_summary_histogram below.
  *
+ * Generated quantities: on a handle whose model has G > 0 (dhmc_generated_count), every array below has R = D + G rows
+ * in place of D — the D parameters, then the G quantities g(θ) of every kept draw, with the same definitions (the shift
+ * of the quantities' sums is g of the position the parameters' shift is).  reference, lo, hi [R, P], record [F, R, P],
+ * counts [nbins + 2, R, P]; dhmc_summary_merge, dhmc_summary_finish and dhmc_histogram_quantiles take R as their row
+ * count.  A non-finite g(θ) is folded as it is and sets no status bit.
+ *
  * The record is [DHMC_SUMMARY_FIELDS, D, P] column-major (the fields of (d, p) at (p·D + d)·F) and holds mergeable
  * quantities in absolute terms: the records of shards of one run (handles with different chain_offset, ranks) combine with
  * dhmc_summary_merge into the record one handle holding every chain would produce, up to rounding. */
@@ -248,7 +271,8 @@ enum {
 };
 /* reference: host [D, P] or NULL; record: host [DHMC_SUMMARY_FIELDS, D, P]; stats / logdens: host [N/thin, B] or NULL (the
  * kept transitions, as dhmc_mcmc_thinned).  DHMC_EARG before anything runs for N < 1, thin < 1, N % thin ≠ 0,
- * N / thin < 4 or record == NULL.  Device memory: one grow-only arena of 8·P·D + 3·D·(resident chain groups) + P doubles.
+ * N / thin < 4 or record == NULL.  Device memory: one grow-only arena of 8·P·D + 3·D·(resident chain groups) + P doubles;
+ * with G generated quantities 8·P·R + (3·D + 5·G)·(resident chain groups) + P doubles.
  * On DHMC_ENUMERIC the record is still written, without the chains that failed. */
 int dhmc_mcmc_summary(dhmc_handle* h, int32_t N, int32_t thin, const double* reference, double* record,
                       dhmc_tree_stats* stats, double* logdens);
@@ -290,7 +314,7 @@ int dhmc_summary_finish(const double* record, int64_t D, int64_t P, double* mean
  * and record) that also writes counts.  lo, hi: host [D, P]; counts: host int64 [nbins + 2, D, P].  DHMC_EARG before
  * anything runs for an invalid grid or nbins, counts == NULL, or any argument dhmc_mcmc_summary rejects.  Device memory
  * on top of dhmc_mcmc_summary's arena: 8·P·D·(nbins + 4) + 4·D·(nbins + 2)·(resident chain groups) bytes (the problem
- * histograms and the grid, and a staging histogram per resident chain group). */
+ * histograms and the grid, and a staging histogram per resident chain group); with G generated quantities R in place of D. */
 int dhmc_mcmc_summary_histogram(dhmc_handle* h, int32_t N, int32_t thin, const double* reference, const double* lo,
                                 const double* hi, int32_t nbins, double* record, int64_t* counts, dhmc_tree_stats* stats,
                                 double* logdens);

@@ -125,7 +125,22 @@ DHMC_HD double dhmc_logit_grad(double xtr, double beta) { return xtr - beta; }
  * it needs to find its data, in the block itself.  The sums are taken in the canonical
  * order (DESIGN.md §3); transcendental functions should come from dhmc_math.h (dm_exp, dm_log, dm_log1p, …) if the
  * device results are to equal the oracle's bit for bit — libm / libdevice calls work, but differ in the last ulp.
- * -Inf / non-finite values are handled by the sampler exactly as for the shipped families (hamiltonian.jl:202-217). */
+ * -Inf / non-finite values are handled by the sampler exactly as for the shipped families (hamiltonian.jl:202-217).
+ *
+ * Generated quantities (optional): functions of one position that the streaming summary reports beside the parameters
+ * (Stan's generated quantities without randomness; e.g. the centred effects of a non-centred model):
+ *
+ *   #define DHMC_USER_GENERATED 1          // absent: the model has none
+ *   DHMC_HD int    dhmc_user_ngq(int D);   // G(D): 1 <= G <= 8192, a function of the dimension only
+ *   // quantity k (0 <= k < G) of the WHOLE position q; params as for dhmc_user_terms (the point's own problem block)
+ *   DHMC_HD double dhmc_user_generated(int k, int D, const double* q, const double* params);
+ *
+ * G may depend on D, not on the parameters, so that every problem of a batch has the same G rows.  Generated quantities
+ * never affect sampling: the draws, statistics, final state and transition counts are those of the same model without
+ * them.  A non-finite value is folded as it is (NaN lands in the top histogram bin and is never below a reference) and
+ * sets no chain status bit.  dhmc_generated evaluates them at given points; dhmc_mcmc_summary appends them to the
+ * parameters as rows D … D + G − 1 (include/dhmc.h).  Where DHMC_USER_NGQ_CONST is defined as G, the bounds are checked
+ * at compile time; otherwise dhmc_create checks G(D). */
 #ifdef DHMC_USER_MODEL_HEADER
 #include DHMC_USER_MODEL_HEADER
 #ifndef DHMC_USER_NSUMS
@@ -142,6 +157,12 @@ DHMC_HD double dhmc_logit_grad(double xtr, double beta) { return xtr - beta; }
 #endif
 #if DHMC_USER_NSUMS < 0 || DHMC_USER_NSUMS > 4 || DHMC_USER_NSCALARS < 0 || DHMC_USER_NSCALARS > 4
 #error "user model header: 0 <= DHMC_USER_NSUMS <= 4 and 0 <= DHMC_USER_NSCALARS <= 4"
+#endif
+#if defined(DHMC_USER_NGQ_CONST) && (DHMC_USER_NGQ_CONST < 1 || DHMC_USER_NGQ_CONST > 8192)   /* DHMC_MAX_GENERATED */
+#error "user model header: 1 <= DHMC_USER_NGQ_CONST <= 8192"
+#endif
+#if defined(DHMC_USER_NGQ_CONST) && !defined(DHMC_USER_GENERATED)
+#error "user model header: DHMC_USER_NGQ_CONST without DHMC_USER_GENERATED"
 #endif
 #define DHMC_HAVE_USER_FAMILY 1
 #endif

@@ -336,11 +336,29 @@ end
 
 # ---- streaming posterior summary (dhmc_mcmc_summary, include/dhmc.h; DESIGN.md §4.4) ----------------------------------
 const SUMMARY_FIELDS = 7
+"G: the generated quantities of the handle's user model (include/dhmc_models.h; dhmc_generated_count), 0 without them."
+function generated_count(h::Handle)
+    G = Ref{Int32}(0)
+    _ck(h, ccall((:dhmc_generated_count, LIB), Cint, (Ptr{Cvoid}, Ptr{Int32}), h.ptr, G))
+    Int(G[])
+end
+"""The generated quantities [G, n, n_problems] of positions θ [D, n, n_problems] (dhmc_generated, on the device): problem
+`first_problem + j` (0-based) lends its parameter block to θ[:, :, j + 1].  Draws [D, N, chains] of a handle holding whole
+problems are θ with n = N·chains per problem; references [D, P] are θ with n = 1."""
+function generated(h::Handle, θ::AbstractArray{Float64}; n::Integer = size(θ, 2), first_problem::Integer = 0,
+                   n_problems::Integer = length(θ) ÷ (h.D * n))
+    G = generated_count(h)
+    out = Array{Float64}(undef, G, n, n_problems)
+    _ck(h, ccall((:dhmc_generated, LIB), Cint, (Ptr{Cvoid}, Ptr{Float64}, Int64, Int64, Int64, Ptr{Float64}),
+                 h.ptr, convert(Array{Float64}, θ), n, first_problem, n_problems, out))
+    out
+end
 """N transitions at the adapted (κ, ϵ), every `thin`-th folded on the device into per-(parameter, problem) statistics; no draw
 is returned.  `reference` [D, P] adds the SBC ranks.  Returns the mergeable record [SUMMARY_FIELDS, D, P] (merge shards with
-`summary_merge!`, finish with `summary_finish`)."""
+`summary_merge!`, finish with `summary_finish`).  A model with G generated quantities has D + G rows in place of D: the
+parameters, then the quantities (`reference` [D + G, P])."""
 function mcmc_summary(h::Handle, N::Integer, P::Integer; thin::Integer = 1, reference = nothing)
-    record = Array{Float64}(undef, SUMMARY_FIELDS, h.D, P)
+    record = Array{Float64}(undef, SUMMARY_FIELDS, h.D + generated_count(h), P)
     ref = reference === nothing ? C_NULL : convert(Matrix{Float64}, reference)
     _ck(h, ccall((:dhmc_mcmc_summary, LIB), Cint, (Ptr{Cvoid}, Int32, Int32, Ptr{Float64}, Ptr{Float64}, Ptr{Cvoid}, Ptr{Float64}),
                  h.ptr, N, thin, ref, record, C_NULL, C_NULL))
@@ -366,11 +384,13 @@ function summary_finish(record::Array{Float64,3})
 end
 """`mcmc_summary` that also counts the kept draws into `nbins` bins of the grid `lo`, `hi` [D, P] plus a tail bin on each side
 (dhmc_mcmc_summary_histogram) and returns `(; record, counts, q, q_lo, q_hi)`: counts [nbins + 2, D, P] (shards on one grid
-add), and the bracketed quantiles [length(quantiles), D, P] of `histogram_quantiles`."""
+add), and the bracketed quantiles [length(quantiles), D, P] of `histogram_quantiles`.  With G generated quantities every D
+is D + G, as above."""
 function mcmc_summary(h::Handle, N::Integer, P::Integer, lo::AbstractMatrix, hi::AbstractMatrix; quantiles,
                       nbins::Integer = 256, thin::Integer = 1, reference = nothing)
-    record = Array{Float64}(undef, SUMMARY_FIELDS, h.D, P)
-    counts = zeros(Int64, nbins + 2, h.D, P)
+    R = h.D + generated_count(h)
+    record = Array{Float64}(undef, SUMMARY_FIELDS, R, P)
+    counts = zeros(Int64, nbins + 2, R, P)
     lo, hi = convert(Matrix{Float64}, lo), convert(Matrix{Float64}, hi)
     ref = reference === nothing ? C_NULL : convert(Matrix{Float64}, reference)
     _ck(h, ccall((:dhmc_mcmc_summary_histogram, LIB), Cint,
