@@ -33,6 +33,7 @@ EXPORTS = [
     "dhmc_allgather_positions_dev", "dhmc_last_comm_ms",
     "dhmc_mcmc_summary", "dhmc_summary_merge", "dhmc_summary_finish", "dhmc_mcmc_summary_histogram",
     "dhmc_histogram_quantiles", "dhmc_generated_count", "dhmc_user_generated_count", "dhmc_generated", "dhmc_generated_dev",
+    "dhmc_generated_random", "dhmc_user_generated_random", "dhmc_generated_keyed", "dhmc_generated_keyed_dev",
 ]
 # streaming summary record (include/dhmc.h DHMC_SUMMARY_*): numpy [P, D, SUMMARY_FIELDS] = column-major [F, D, P]
 (SUMMARY_CHAINS, SUMMARY_NKEEP, SUMMARY_MEAN, SUMMARY_SS_SEQ, SUMMARY_M2, SUMMARY_SS_CHAIN, SUMMARY_BELOW,
@@ -82,6 +83,12 @@ def lib(path=None):
         so.dhmc_user_generated_count.argtypes = [C.c_int64, C.c_void_p]
         so.dhmc_generated.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p]
         so.dhmc_generated_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p]
+        so.dhmc_generated_random.argtypes = [C.c_void_p, C.c_void_p]
+        so.dhmc_user_generated_random.argtypes = [C.c_void_p]
+        so.dhmc_generated_keyed.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p,
+                                            C.c_void_p]
+        so.dhmc_generated_keyed_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p,
+                                                C.c_void_p]
         _libs[path] = so
     return so
 

@@ -234,6 +234,14 @@ class UserLogDensity(DeviceLogDensity):
                   f"{self.library_path} carries no user model")
         return G.value
 
+    def generated_random(self):
+        """1 when the header's generated quantities are random (DHMC_USER_GENERATED_RNG: posterior predictive replicates,
+        evaluated with a key per draw; Engine.generated(..., keys=...)), else 0."""
+        r = C.c_int32()
+        _argcheck(L.lib(self.library_path).dhmc_user_generated_random(C.byref(r)) == L.DHMC_OK,
+                  f"{self.library_path} carries no user model")
+        return r.value
+
     def model_name(self):
         buf = C.create_string_buffer(128)
         rc = L.lib(self.library_path).dhmc_user_family_name(buf, C.c_size_t(128))
@@ -427,6 +435,7 @@ class GaussianKineticEnergy:
 class Engine:
     """Owns a dhmc_handle: K chains of one problem (or of a ProblemBatch) on one GPU."""
     _G = 0            # generated quantities of the handle's model (dhmc_generated_count, set per handle)
+    _GR = 0           # 1: they are random (dhmc_generated_random)
 
     def __init__(self, ℓ: DeviceLogDensity, chains: int, seed: int = 0, algorithm: NUTS = None,
                  device: int = 0, chain_offset: int = 0, threads_per_chain: int = 0,
@@ -451,6 +460,8 @@ class Engine:
         G = C.c_int32()
         self._ck(self._lib.dhmc_generated_count(h, C.byref(G)))
         self._G = G.value
+        self._ck(self._lib.dhmc_generated_random(h, C.byref(G)))
+        self._GR = G.value
         self._set_problem(ℓ)
 
     def _set_problem(self, ℓ):
@@ -706,22 +717,70 @@ class Engine:
         """G: the generated quantities of the handle's model (a user model with DHMC_USER_GENERATED), 0 without them."""
         return self._G
 
+    @property
+    def generated_random(self):
+        """1 when the model's generated quantities are random (DHMC_USER_GENERATED_RNG), else 0: generated then needs keys,
+        and mcmc_summary a reference of all D + G rows."""
+        return self._GR
+
     def _n_problems(self):
         return self.ℓ.n_problems if isinstance(self.ℓ, ProblemBatch) else 1
 
-    def generated(self, theta, problem=None):
+    def draw_keys(self, t0, N, thin=1):
+        """The keys (chain ids, transitions), each [K, N // thin], of the posterior_matrix of a call of N transitions with
+        thinning `thin` that started at transition count t0 (transition_count before the call): kept draw j of chain k was
+        produced by transition t0 + (j + 1)·thin − 1 of global chain chain_offset + k.  With them, generated(post, keys=...)
+        reproduces the random quantities the summary folded for those draws."""
+        _argcheck(thin >= 1 and N >= thin and N % thin == 0, "thin ≥ 1 and N a positive multiple of thin")
+        _argcheck(int(t0) == t0 and 0 <= t0 < 2 ** 32, "t0: a transition count in [0, 2^32)")
+        n = N // thin
+        chain = np.broadcast_to((self.chain_offset + np.arange(self.K, dtype=np.int64))[:, None], (self.K, n))
+        trans = (int(t0) + (np.arange(n, dtype=np.int64) + 1) * int(thin) - 1) % (2 ** 32)
+        return np.ascontiguousarray(chain), np.ascontiguousarray(np.broadcast_to(trans.astype(np.uint32), (self.K, n)))
+
+    def _keys(self, keys, shape):
+        """(chain ids int64, transitions uint32), each of `shape`, from a pair broadcastable to it"""
+        _argcheck(isinstance(keys, (tuple, list)) and len(keys) == 2, "keys: (chain ids, transitions)")
+        out = []
+        for a, name, hi in ((keys[0], "chain ids", 2 ** 56), (keys[1], "transitions", 2 ** 32)):
+            a = np.asarray(a)
+            _argcheck(a.dtype.kind in "iu" or (a.dtype.kind == "f" and np.all(a == np.floor(a))), f"keys: integral {name}")
+            try:
+                a = np.broadcast_to(a, shape)
+            except ValueError:
+                raise ArgumentError(f"keys: {name} of shape {a.shape} do not broadcast to the points' shape {shape}") from None
+            _argcheck(np.all((a >= 0) & (a < hi)), f"keys: {name} in [0, {hi})")
+            out.append(np.ascontiguousarray(a, np.int64 if hi == 2 ** 56 else np.uint32))
+        return out
+
+    def generated(self, theta, problem=None, keys=None):
         """The G generated quantities of positions `theta` (numpy; dhmc_generated, evaluated on the device) with the last
         axis G in place of D.  Each point reads the parameter block of its problem:
           [D]          one point of `problem` (default 0)
           [n, D]       n points of `problem`; without one, of problem 0 on a one-problem handle, else one point per
                        problem (n = P: per-problem references)
           [K, N, D]    the posterior_matrix of mcmc: chain k's draws read the problem of global chain chain_offset + k,
-                       or all read `problem`"""
+                       or all read `problem`
+
+        Random quantities (generated_random) need `keys` = (chain ids, transitions), integer arrays broadcastable to
+        theta.shape[:-1] (draw_keys gives those of a posterior_matrix; dhmc_generated_keyed).  A deterministic model
+        accepts keys and ignores them."""
         _argcheck(self._G > 0, "the model has no generated quantities (include/dhmc_models.h DHMC_USER_GENERATED)")
+        _argcheck(keys is not None or not self._GR,
+                  "the model's generated quantities are random: pass keys = (chain ids, transitions) (Engine.draw_keys)")
         th = np.ascontiguousarray(theta, float)
         _argcheck(th.ndim in (1, 2, 3) and th.shape[-1] == self.D, f"theta: [..., D] with D = {self.D}")
         P, G = self._n_problems(), self._G
         out = np.empty(th.shape[:-1] + (G,))
+        kc, kt = self._keys(keys, th.shape[:-1]) if keys is not None else (None, None)
+
+        def call(first_pt, n, p, n_problems):                              # points first_pt … of problems p … p + n_problems − 1
+            at, o = th.reshape(-1, self.D)[first_pt:], out.reshape(-1, G)[first_pt:]
+            if kc is None:
+                self._ck(self._lib.dhmc_generated(self._h, L.ptr(at), n, p, n_problems, L.ptr(o)))
+            else:
+                self._ck(self._lib.dhmc_generated_keyed(self._h, L.ptr(at), n, p, n_problems, L.ptr(kc.reshape(-1)[first_pt:]),
+                                                        L.ptr(kt.reshape(-1)[first_pt:]), L.ptr(o)))
         if problem is not None:
             _argcheck(int(problem) == problem and 0 <= problem < P, f"problem: 0 … {P - 1}")
             runs = [(int(problem), 0, th.size // self.D)]                     # (problem, first point, points)
@@ -737,17 +796,16 @@ class Engine:
                 else:
                     runs.append([int(prob[k]), k * N, N])
             if len({r[2] for r in runs}) == 1 and len(runs) > 1:          # whole problems: one call over all of them
-                self._ck(self._lib.dhmc_generated(self._h, L.ptr(th), runs[0][2], runs[0][0], len(runs), L.ptr(out)))
+                call(0, runs[0][2], runs[0][0], len(runs))
                 return out
         elif th.ndim == 2 and P > 1:
             _argcheck(th.shape[0] == P, f"theta [n, D] without a problem: one point per problem (n = P = {P})")
-            self._ck(self._lib.dhmc_generated(self._h, L.ptr(th), 1, 0, P, L.ptr(out)))
+            call(0, 1, 0, P)
             return out
         else:
             runs = [(0, 0, th.size // self.D)]
-        flat, fout = th.reshape(-1, self.D), out.reshape(-1, G)
         for p, first, n in runs:
-            self._ck(self._lib.dhmc_generated(self._h, L.ptr(flat[first:]), n, p, 1, L.ptr(fout[first:])))
+            call(first, n, p, 1)
         return out
 
     def mcmc_summary(self, N, thin=1, reference=None, stats=False, quantiles=None, grid=None, bins=256):
@@ -768,7 +826,9 @@ class Engine:
 
         A model with G generated quantities (generated_count) is summarized on R = D + G rows: the D parameters, then the
         G quantities of every kept draw.  Every [P, D] above is then [P, R]; a `reference` [P, D] is extended with its
-        generated quantities (Engine.generated), one [P, R] is taken as given."""
+        generated quantities (Engine.generated), one [P, R] is taken as given.  Random quantities (generated_random) are
+        ordinary rows, each kept draw evaluated under its own key (draw_keys); g(reference) is random there, so such a
+        model takes only a [P, R] reference (a NaN cell counts nothing)."""
         from . import diagnostics
         _argcheck(N >= 1 and thin >= 1 and N % thin == 0, "N ≥ 1, thin ≥ 1 and N a multiple of thin")
         _argcheck(N // thin >= 4, "at least 4 kept draws per chain (N / thin ≥ 4)")
@@ -777,7 +837,10 @@ class Engine:
         ref = None
         if reference is not None:
             ref = np.ascontiguousarray(reference, float)
-            if self._G:
+            if self._GR:
+                _argcheck(ref.shape == (P, R), f"reference: [P, D + G] = ({P}, {R}); the model's generated quantities are "
+                                               "random, so g(reference) is not defined by the reference: give all rows")
+            elif self._G:
                 _argcheck(ref.shape in ((P, self.D), (P, R)), f"reference: [P, D] = ({P}, {self.D}) or [P, D + G] = ({P}, {R})")
                 if ref.shape == (P, self.D):
                     ref = np.ascontiguousarray(np.concatenate([ref, self.generated(ref)], axis=1))

@@ -51,10 +51,13 @@ const void* dhmc_user_family_kernel_0(int W, int epl, int kernel, int dense) DHM
 const void* dhmc_user_family_kernel_3(int W, int epl, int kernel, int dense) DHMC_TU_LINKAGE;
 const char* dhmc_user_family_name_str(void) DHMC_TU_LINKAGE;
 int dhmc_user_family_min_dim(void) DHMC_TU_LINKAGE;
-// generated quantities (a model with DHMC_USER_GENERATED): G(D) and the launch of k_generated (family_tu.cu)
+// generated quantities (a model with DHMC_USER_GENERATED): G(D), whether they are random (DHMC_USER_GENERATED_RNG) and
+// the launch of k_generated (family_tu.cu)
 int dhmc_user_family_ngq(int D) DHMC_TU_LINKAGE;
+int dhmc_user_family_random(void) DHMC_TU_LINKAGE;
 int dhmc_user_family_generated(const double* theta, long long n, long long n_problems, int D, int ng, const double* mparams,
-                               const void* problems, long long first, double* out, int T, int grid, cudaStream_t stream) DHMC_TU_LINKAGE;
+                               const void* problems, long long first, const long long* chain, const unsigned* transition,
+                               unsigned long long seed, double* out, int T, int grid, cudaStream_t stream) DHMC_TU_LINKAGE;
 }
 // part: 0 = one chain per CTA, 1 = packed chain groups (likelihood on the tensor cores),
 // 3 = one chain per CTA with max_depth > 12 (persistent kernels only)
@@ -368,6 +371,7 @@ struct dhmc_handle {
   size_t sum_bytes = 0;
   SummaryArgs* sum_args = nullptr;
   int ngq = 0;                      // generated quantities of a user model (dhmc_generated_count)
+  bool gq_random = false;           // ... drawn from the keyed streams (dhmc_generated_random)
   std::string err;
 };
 
@@ -666,6 +670,7 @@ int dhmc_create(const dhmc_config* cfg, dhmc_handle** out) {
   dhmc_handle* h = new dhmc_handle();
   h->cfg = *cfg; h->T = T; h->W = T / 32; h->EPL = EPL; h->stride = (size_t)T * EPL; h->G = pack; h->deep = deep;
   h->ngq = ngq;
+  h->gq_random = ngq > 0 && dhmc_user_family_random && dhmc_user_family_random() != 0;
   h->n_slots = slots_needed(cfg->max_depth);
   h->levels = deep ? cfg->max_depth + 1 : kStdLevels;        // deep persistent kernels size their stack / slot table at run time
   h->ntab = deep ? std::max(kStdTab, (h->n_slots + 7) & ~7) : kStdTab;
@@ -1416,23 +1421,34 @@ static cudaError_t upload_rows(double* dst, const double* src, size_t r0, size_t
 }
 
 // generated quantities of device points theta [n_problems][n][D] (problem first + j owns points j·n … (j+1)·n − 1) into
-// out [n_problems][n][G] on the handle's stream (k_generated, family_tu.cu); the caller has checked the arguments
-static int launch_generated(dhmc_handle* h, const double* theta, int64_t n, int64_t first, int64_t n_problems, double* out) {
+// out [n_problems][n][G] on the handle's stream (k_generated, family_tu.cu); random quantities read point pt's key from the
+// device arrays chain [pt] and transition [pt] (null for deterministic ones); the caller has checked the arguments
+static int launch_generated(dhmc_handle* h, const double* theta, int64_t n, int64_t first, int64_t n_problems, const int64_t* chain,
+                            const uint32_t* transition, double* out) {
   const int64_t pts = n * n_problems;
   const int grid = (int)std::min<int64_t>(pts, (int64_t)h->sm_count * 16);
   const int e = dhmc_user_family_generated(theta, n, n_problems, (int)h->cfg.dim, h->ngq, h->mparams,
-                                           h->batch_k ? h->problems : nullptr, first, out, h->T, grid, h->stream);
+                                           h->batch_k ? h->problems : nullptr, first, (const long long*)chain, transition,
+                                           (unsigned long long)h->cfg.seed, out, h->T, grid, h->stream);
   if (e != cudaSuccess) { h->err = std::string("k_generated: ") + cudaGetErrorString((cudaError_t)e); return DHMC_ECUDA; }
   h->launches += 1;
   return DHMC_OK;
 }
 
-// dhmc_generated(_dev): DHMC_EARG before anything runs for a handle without generated quantities, NULL pointers, n < 1,
-// n_problems < 1 or a problem range outside the handle's batch
-static int check_generated(dhmc_handle* h, const double* theta, int64_t n, int64_t first, int64_t n_problems, const double* out) {
+// dhmc_generated(_dev) and dhmc_generated_keyed(_dev): DHMC_EARG before anything runs for a handle without generated
+// quantities, NULL pointers, n < 1, n_problems < 1, a problem range outside the handle's batch, or a model with random
+// quantities called without keys
+static int check_generated(dhmc_handle* h, const double* theta, int64_t n, int64_t first, int64_t n_problems, const double* out,
+                           bool keyed, const int64_t* chain, const uint32_t* transition) {
   const int64_t P = h->batch_k ? h->batch_p : 1;
   if (h->ngq == 0) { h->err = "dhmc_generated: the handle's model has no generated quantities"; return DHMC_EARG; }
+  if (!keyed && h->gq_random) {
+    h->err = "dhmc_generated: the model's generated quantities are random (DHMC_USER_GENERATED_RNG); call dhmc_generated_keyed "
+             "with the chain id and transition of every point";
+    return DHMC_EARG;
+  }
   if (!theta || !out) { h->err = "dhmc_generated: theta or out is NULL"; return DHMC_EARG; }
+  if (keyed && (!chain || !transition)) { h->err = "dhmc_generated_keyed: chain or transition is NULL"; return DHMC_EARG; }
   if (n < 1 || n_problems < 1 || first < 0 || first > P - n_problems) {
     h->err = "dhmc_generated: n ≥ 1, and problems first … first + n_problems − 1 of the handle's batch";
     return DHMC_EARG;
@@ -1446,39 +1462,81 @@ int dhmc_user_generated_count(int64_t dim, int32_t* G) {
   return DHMC_OK;
 }
 
+int dhmc_user_generated_random(int32_t* random) {
+  if (!dhmc_user_family_name_str || !random) return DHMC_EARG;
+  *random = dhmc_user_family_random ? dhmc_user_family_random() : 0;
+  return DHMC_OK;
+}
+
 int dhmc_generated_count(dhmc_handle* h, int32_t* G) {
   if (!h || !G) return DHMC_EARG;
   *G = h->ngq;
   return DHMC_OK;
 }
 
-int dhmc_generated_dev(dhmc_handle* h, const double* theta, int64_t n, int64_t first_problem, int64_t n_problems, double* out) {
+int dhmc_generated_random(dhmc_handle* h, int32_t* random) {
+  if (!h || !random) return DHMC_EARG;
+  *random = h->gq_random ? 1 : 0;
+  return DHMC_OK;
+}
+
+// device arrays: check, launch, wait
+static int generated_dev(dhmc_handle* h, const double* theta, int64_t n, int64_t first, int64_t n_problems, bool keyed,
+                         const int64_t* chain, const uint32_t* transition, double* out) {
   if (!h) return DHMC_EARG;
-  const int rc = check_generated(h, theta, n, first_problem, n_problems, out);
+  const int rc = check_generated(h, theta, n, first, n_problems, out, keyed, chain, transition);
   if (rc != DHMC_OK) return rc;
   CK(cudaSetDevice(h->cfg.device));
-  const int rg = launch_generated(h, theta, n, first_problem, n_problems, out);
+  const int rg = launch_generated(h, theta, n, first, n_problems, chain, transition, out);
   if (rg != DHMC_OK) return rg;
   CK(cudaStreamSynchronize(h->stream));
   return DHMC_OK;
 }
 
-int dhmc_generated(dhmc_handle* h, const double* theta, int64_t n, int64_t first_problem, int64_t n_problems, double* out) {
+// host arrays: check (keys: chain ids in [0, 2^56), the key's width), upload points and keys, launch, download
+static int generated_host(dhmc_handle* h, const double* theta, int64_t n, int64_t first, int64_t n_problems, bool keyed,
+                          const int64_t* chain, const uint32_t* transition, double* out) {
   if (!h) return DHMC_EARG;
-  const int rc = check_generated(h, theta, n, first_problem, n_problems, out);
+  const int rc = check_generated(h, theta, n, first, n_problems, out, keyed, chain, transition);
   if (rc != DHMC_OK) return rc;
-  CK(cudaSetDevice(h->cfg.device));
   const size_t pts = (size_t)n * (size_t)n_problems, D = (size_t)h->cfg.dim, G = (size_t)h->ngq;
+  if (keyed)
+    for (size_t i = 0; i < pts; ++i)
+      if (chain[i] < 0 || chain[i] >= ((int64_t)1 << 56)) { h->err = "dhmc_generated_keyed: chain ids lie in [0, 2^56)"; return DHMC_EARG; }
+  CK(cudaSetDevice(h->cfg.device));
+  // one buffer: points [pts][D], out [pts][G], then with keys chain [pts] (8-byte) and transition [pts] (4-byte)
   double* buf = nullptr;
-  CK(cudaMalloc(&buf, sizeof(double) * pts * (D + G)));
+  CK(cudaMalloc(&buf, sizeof(double) * pts * (D + G) + (keyed ? (sizeof(int64_t) + sizeof(uint32_t)) * pts : 0)));
+  int64_t* dchain = keyed ? (int64_t*)(buf + pts * (D + G)) : nullptr;
+  uint32_t* dtrans = keyed ? (uint32_t*)(dchain + pts) : nullptr;
   cudaError_t e = cudaMemcpyAsync(buf, theta, sizeof(double) * pts * D, cudaMemcpyHostToDevice, h->stream);
-  int rg = e == cudaSuccess ? launch_generated(h, buf, n, first_problem, n_problems, buf + pts * D) : DHMC_OK;
+  if (keyed && e == cudaSuccess) e = cudaMemcpyAsync(dchain, chain, sizeof(int64_t) * pts, cudaMemcpyHostToDevice, h->stream);
+  if (keyed && e == cudaSuccess) e = cudaMemcpyAsync(dtrans, transition, sizeof(uint32_t) * pts, cudaMemcpyHostToDevice, h->stream);
+  int rg = e == cudaSuccess ? launch_generated(h, buf, n, first, n_problems, dchain, dtrans, buf + pts * D) : DHMC_OK;
   if (e == cudaSuccess && rg == DHMC_OK)
     e = cudaMemcpyAsync(out, buf + pts * D, sizeof(double) * pts * G, cudaMemcpyDeviceToHost, h->stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
   cudaFree(buf);
   if (e != cudaSuccess) { h->err = std::string("dhmc_generated: ") + cudaGetErrorString(e); return DHMC_ECUDA; }
   return rg;
+}
+
+int dhmc_generated_dev(dhmc_handle* h, const double* theta, int64_t n, int64_t first_problem, int64_t n_problems, double* out) {
+  return generated_dev(h, theta, n, first_problem, n_problems, false, nullptr, nullptr, out);
+}
+
+int dhmc_generated(dhmc_handle* h, const double* theta, int64_t n, int64_t first_problem, int64_t n_problems, double* out) {
+  return generated_host(h, theta, n, first_problem, n_problems, false, nullptr, nullptr, out);
+}
+
+int dhmc_generated_keyed(dhmc_handle* h, const double* theta, int64_t n, int64_t first_problem, int64_t n_problems,
+                         const int64_t* chain, const uint32_t* transition, double* out) {
+  return generated_host(h, theta, n, first_problem, n_problems, true, chain, transition, out);
+}
+
+int dhmc_generated_keyed_dev(dhmc_handle* h, const double* theta, int64_t n, int64_t first_problem, int64_t n_problems,
+                             const int64_t* chain, const uint32_t* transition, double* out) {
+  return generated_dev(h, theta, n, first_problem, n_problems, true, chain, transition, out);
 }
 
 // dhmc_mcmc_summary and, with counts, dhmc_mcmc_summary_histogram (arguments checked by the caller)
@@ -1503,8 +1561,11 @@ static int mcmc_summary(dhmc_handle* h, int32_t N, int32_t thin, const double* r
   // one grow-only arena: acc [P][5][D], shift [P][D], ref [P][D], row [grid·G][3][D], below [P][D], chains [P], then with
   // histograms hist [P][D][cells], lo [P][D], inv_w [P][D]; the same for the generated quantities (gacc, gshift, gref, grow,
   // gbelow, ghist, glo, ginv_w; 8-byte elements); last stage [grid·G][cells][D] and gstage [grid·G][cells][ng] (4-byte)
-  const size_t need = sizeof(double) * (8 * PD + rows + P + PD * cells + (counts ? 2 * PD : 0)) + sizeof(unsigned) * stage +
+  // random generated quantities: last the keys of the shift's points, chain [P] (8-byte) and transition [P] (4-byte), 8-aligned
+  const size_t body = sizeof(double) * (8 * PD + rows + P + PD * cells + (counts ? 2 * PD : 0)) + sizeof(unsigned) * stage +
                       sizeof(double) * (8 * PG + grows + PG * cells + (counts ? 2 * PG : 0)) + sizeof(unsigned) * gstage;
+  const size_t keys_at = (body + 7) & ~(size_t)7;
+  const size_t need = h->gq_random ? keys_at + (sizeof(int64_t) + sizeof(uint32_t)) * P : body;
   if (need > h->sum_bytes) {
     cudaFree(h->sum_buf); h->sum_buf = nullptr; h->sum_bytes = 0;
     CK(cudaMalloc(&h->sum_buf, need));
@@ -1551,10 +1612,25 @@ static int mcmc_summary(dhmc_handle* h, int32_t N, int32_t thin, const double* r
   if (ng) {
     CK(cudaMemsetAsync(gacc, 0, sizeof(double) * 5 * PG, h->stream));
     CK(cudaMemsetAsync(gbelow, 0, sizeof(unsigned long long) * PG, h->stream));
-    const int rg = launch_generated(h, shift + p0 * D, 1, p0, p1 - p0 + 1, gshift + p0 * ng);
+    // random quantities: the shift's key is (global id of the problem's first local chain, the call's first transition);
+    // it only sets the cancellation shift of the sums
+    int64_t* kchain = nullptr;
+    uint32_t* ktrans = nullptr;
+    if (h->gq_random) {
+      const size_t np = (size_t)(p1 - p0 + 1);
+      kchain = (int64_t*)((char*)h->sum_buf + keys_at);
+      ktrans = (uint32_t*)(kchain + np);
+      std::vector<int64_t> hc(np);
+      std::vector<uint32_t> ht(np, h->t);
+      for (size_t i = 0; i < np; ++i) hc[i] = K ? std::max((p0 + (int64_t)i) * K, off) : off;
+      CK(cudaMemcpyAsync(kchain, hc.data(), sizeof(int64_t) * np, cudaMemcpyHostToDevice, h->stream));
+      CK(cudaMemcpyAsync(ktrans, ht.data(), sizeof(uint32_t) * np, cudaMemcpyHostToDevice, h->stream));
+    }
+    const int rg = launch_generated(h, shift + p0 * D, 1, p0, p1 - p0 + 1, kchain, ktrans, gshift + p0 * ng);
     if (rg != DHMC_OK) return rg;
     if (reference) CK(upload_rows(gref, reference, D, ng, R, P, h->stream));
     sa.ng = (int)ng; sa.mparams = h->mparams; sa.problems = K ? h->problems : nullptr;
+    sa.seed = (unsigned long long)h->cfg.seed; sa.chain_offset = (long long)off; sa.t0 = h->t; sa.thin = thin;
     sa.grow = grow; sa.gshift = gshift; sa.gref = reference ? gref : nullptr; sa.gacc = gacc; sa.gbelow = gbelow;
     if (counts) {
       double* glo = (double*)(ghist + PG * cells);

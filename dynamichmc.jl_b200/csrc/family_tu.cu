@@ -29,23 +29,41 @@ extern "C" __attribute__((visibility("hidden"))) int dhmc_user_family_min_dim(vo
 #ifdef DHMC_USER_GENERATED
 // Generated quantities at given points (dhmc_generated): one CTA of T threads (the handle's chain width) per point, thread
 // tid writing quantities k = tid + e·T.  theta [n_problems][n][D], out [n_problems][n][G]; the points of local problem j
-// read the parameter block of problem first + j (problems null: the handle's one problem).
+// read the parameter block of problem first + j (problems null: the handle's one problem).  Random quantities
+// (DHMC_USER_GENERATED_RNG) take point pt's key from chain [pt] and transition [pt] under `seed`; deterministic ones
+// ignore the keys (null).
 namespace dhmc {
 __global__ void k_generated(const double* theta, long long n, long long n_problems, int D, int ng, const double* mparams,
-                            const ProblemDesc* problems, long long first, double* out) {
+                            const ProblemDesc* problems, long long first, const long long* chain, const unsigned* transition,
+                            unsigned long long seed, double* out) {
   for (long long pt = blockIdx.x; pt < n * n_problems; pt += gridDim.x) {
     const double* params = mparams + (problems ? problems[first + pt / n].mparams : 0);
     const double* q = theta + (size_t)pt * D;
+#ifdef DHMC_USER_GENERATED_RNG
+    dhmc_gq_rng rng;
+    rng.key = dm_make_key(seed, (uint64_t)chain[pt]);
+    rng.t = transition[pt];
+    for (int k = threadIdx.x; k < ng; k += blockDim.x) out[(size_t)pt * ng + k] = dhmc_user_generated(k, D, q, params, &rng);
+#else
+    (void)chain; (void)transition; (void)seed;
     for (int k = threadIdx.x; k < ng; k += blockDim.x) out[(size_t)pt * ng + k] = dhmc_user_generated(k, D, q, params);
+#endif
   }
 }
 }  // namespace dhmc
 extern "C" __attribute__((visibility("hidden"))) int dhmc_user_family_ngq(int D) { return dhmc_user_ngq(D); }
+#ifdef DHMC_USER_GENERATED_RNG
+extern "C" __attribute__((visibility("hidden"))) int dhmc_user_family_random(void) { return 1; }
+#else
+extern "C" __attribute__((visibility("hidden"))) int dhmc_user_family_random(void) { return 0; }
+#endif
 extern "C" __attribute__((visibility("hidden"))) int dhmc_user_family_generated(const double* theta, long long n, long long n_problems,
                                                                                 int D, int ng, const double* mparams, const void* problems,
-                                                                                long long first, double* out, int T, int grid,
-                                                                                cudaStream_t stream) {
-  dhmc::k_generated<<<grid, T, 0, stream>>>(theta, n, n_problems, D, ng, mparams, (const dhmc::ProblemDesc*)problems, first, out);
+                                                                                long long first, const long long* chain,
+                                                                                const unsigned* transition, unsigned long long seed,
+                                                                                double* out, int T, int grid, cudaStream_t stream) {
+  dhmc::k_generated<<<grid, T, 0, stream>>>(theta, n, n_problems, D, ng, mparams, (const dhmc::ProblemDesc*)problems, first, chain,
+                                            transition, seed, out);
   return (int)cudaGetLastError();
 }
 #endif

@@ -48,6 +48,8 @@ struct ProblemDesc {
 //   grow   [grid·G][5][ng]  per chain group: the running sequence's mean and M2, sequence 0's mean and M2, the below-count
 //   gshift, gref, gbelow, glo, ginv_w [P][ng];  gacc [P][5][ng];  gstage [grid·G][nbins + 2][ng];  ghist [P][ng][nbins + 2]
 //   mparams, problems   the problem blocks the quantities read (problems null: one problem)
+// Random generated quantities (DHMC_USER_GENERATED_RNG): kept draw j of local chain c has the key (seed, chain_offset + c)
+// and transition t0 + (j + 1)·thin − 1, the RNG counter of the transition that produced it (include/dhmc_models.h).
 struct SummaryArgs {
   double* row;
   const double* shift;
@@ -73,6 +75,10 @@ struct SummaryArgs {
   const double* ginv_w;
   unsigned* gstage;
   unsigned long long* ghist;
+  unsigned long long seed;
+  long long chain_offset;
+  unsigned t0;
+  int thin;
 };
 
 struct KArgs {
@@ -277,9 +283,18 @@ __device__ __forceinline__ void store_vec(const DeviceBackend<EPL, FAM, W, DN, G
 __device__ __forceinline__ size_t summary_problem(const KArgs& a, long c) {
   return a.batch_k ? (size_t)((unsigned)(a.chain_offset + c) / (unsigned)a.batch_k) : 0;
 }
+// Random generated quantities key their numbers by the chain: summary_draw takes the local chain c in those builds only, so
+// that every other build keeps its code.
+#ifdef DHMC_USER_GENERATED_RNG
+#define DHMC_GQ_CHAIN_PARAM , long c
+#define DHMC_GQ_CHAIN_ARG , c
+#else
+#define DHMC_GQ_CHAIN_PARAM
+#define DHMC_GQ_CHAIN_ARG
+#endif
 template <class Bk>
 __device__ __noinline__ void summary_draw(const SummaryArgs* sp, double** slot_tab, int n_slots, int s_zq, int tid, int grp, int D,
-                                         size_t p, int j);
+                                         size_t p, int j DHMC_GQ_CHAIN_PARAM);
 
 template <int EPL, int FAM, int W, bool DN, int G, bool DP>
 struct DrawSink {
@@ -306,7 +321,7 @@ struct DrawSink {
     }
     if (a.summary)
       summary_draw<DeviceBackend<EPL, FAM, W, DN, G, DP>>(a.summary, b.slot_tab, b.n_slots, b.top().s_zq, b.tid, b.grp, a.D,
-                                                          summary_problem(a, c), n);
+                                                          summary_problem(a, c), n DHMC_GQ_CHAIN_ARG);
   }
 };
 
@@ -381,9 +396,11 @@ __device__ __noinline__ void summary_hist_fold(const SummaryArgs* sp, int tid, i
 // other build keeps its code.  Quantity k reads the whole kept position, elements other threads wrote, so the chain
 // synchronises before it reads the slot and again before the next transition may overwrite it (one chain per CTA: the
 // USER family has no packed groups).  Thread tid evaluates and folds k = tid + e·T, with the moments, the rank and the bin
-// rule of the parameters; its state for k lives in grow, and nothing else reads it.
+// rule of the parameters; its state for k lives in grow, and nothing else reads it.  Random quantities get the draw's key:
+// (seed, global chain id) and the counter of the transition that produced kept draw j.
 template <class Bk>
-__device__ __noinline__ void summary_gq_draw(const SummaryArgs* sp, const double* zq, int tid, int grp, int D, size_t p, int j) {
+__device__ __noinline__ void summary_gq_draw(const SummaryArgs* sp, const double* zq, int tid, int grp, int D, size_t p, int j
+                                             DHMC_GQ_CHAIN_PARAM) {
   static_assert(Bk::G == 1, "generated quantities: one chain per CTA");
   constexpr int T = Bk::T;
   const SummaryArgs& s = *sp;
@@ -391,10 +408,19 @@ __device__ __noinline__ void summary_gq_draw(const SummaryArgs* sp, const double
   const double* params = s.mparams + (s.problems ? s.problems[p].mparams : 0);
   double* gr = s.grow + summary_group<Bk>(grp) * 5 * (size_t)ng;
   unsigned* stage = s.ghist ? s.gstage + summary_group<Bk>(grp) * (size_t)(nb + 2) * (size_t)ng : nullptr;
+#ifdef DHMC_USER_GENERATED_RNG
+  dhmc_gq_rng rng;
+  rng.key = dm_make_key(s.seed, (uint64_t)(s.chain_offset + c));
+  rng.t = s.t0 + (unsigned)(j + 1) * (unsigned)s.thin - 1u;
+#endif
   __syncthreads();
 #pragma unroll 1
   for (int k = tid; k < ng; k += T) {
+#ifdef DHMC_USER_GENERATED_RNG
+    const double v = dhmc_user_generated(k, D, zq, params, &rng);
+#else
     const double v = dhmc_user_generated(k, D, zq, params);
+#endif
     if (j < 2 * n) {
       const int kk = j < n ? j + 1 : j - n + 1;        // place in its sequence (1-based); metric_reset / metric_push
       const double mean = kk == 1 ? 0.0 : gr[k], m2 = kk == 1 ? 0.0 : gr[ng + k];
@@ -454,7 +480,7 @@ __device__ __noinline__ void summary_gq_fold(const SummaryArgs* sp, int tid, int
 // kept draw j: sequence 0 is draws [0, n), sequence 1 draws [n, 2n); an odd last draw counts for the rank only
 template <class Bk>
 __device__ __noinline__ void summary_draw(const SummaryArgs* sp, double** slot_tab, int n_slots, int s_zq, int tid, int grp, int D,
-                                         size_t p, int j) {
+                                         size_t p, int j DHMC_GQ_CHAIN_PARAM) {
   constexpr int EPL = sizeof(Bk::q) / sizeof(double), T = Bk::T;
   const SummaryArgs& s = *sp;
   Bk w = welford_view<Bk>(slot_tab, n_slots, tid, D);
@@ -489,7 +515,7 @@ __device__ __noinline__ void summary_draw(const SummaryArgs* sp, double** slot_t
   }
   if (s.hist) summary_hist_draw<Bk>(sp, slot_tab[s_zq] + tid, tid, grp, D, p, j);
 #ifdef DHMC_USER_GENERATED
-  if (s.ng) summary_gq_draw<Bk>(sp, slot_tab[s_zq], tid, grp, D, p, j);
+  if (s.ng) summary_gq_draw<Bk>(sp, slot_tab[s_zq], tid, grp, D, p, j DHMC_GQ_CHAIN_ARG);
 #endif
 }
 // chain end (the chain completed the call): fold its two sequences into its problem's sums

@@ -155,6 +155,22 @@ int dhmc_user_generated_count(int64_t dim, int32_t* G);
 int dhmc_generated(dhmc_handle* h, const double* theta, int64_t n, int64_t first_problem, int64_t n_problems, double* out);
 int dhmc_generated_dev(dhmc_handle* h, const double* theta, int64_t n, int64_t first_problem, int64_t n_problems,
                        double* out);
+/* Random generated quantities (include/dhmc_models.h, DHMC_USER_GENERATED_RNG), e.g. posterior predictive replicates:
+ * *random = 1 when the model's quantities draw numbers from the keyed streams, else 0.  dhmc_user_generated_random needs
+ * no handle (DHMC_EARG in a library without a user model).  dhmc_generated(_dev) refuses such a model with DHMC_EARG. */
+int dhmc_generated_random(dhmc_handle* h, int32_t* random);
+int dhmc_user_generated_random(int32_t* random);
+/* dhmc_generated with a key per point: chain [n, n_problems] (int64 global chain ids) and transition [n, n_problems] (uint32
+ * transition counters), on the same side as theta; point i draws its numbers under (the handle's seed, chain[i]) and
+ * transition[i].  The kept draw j of a sampling call that started at transition count t0 with thinning `thin`, of local
+ * chain c, has chain = chain_offset + c and transition = t0 + (j + 1)·thin − 1 (uint32 arithmetic): with those keys the
+ * quantities equal the summary's.  Layout and problem rules are dhmc_generated's.  DHMC_EARG before anything runs for
+ * NULL keys, any argument dhmc_generated rejects, and (host variant) a chain id outside [0, 2^56).  On a model whose
+ * quantities are deterministic the keys are ignored and the output is dhmc_generated's, bit for bit. */
+int dhmc_generated_keyed(dhmc_handle* h, const double* theta, int64_t n, int64_t first_problem, int64_t n_problems,
+                         const int64_t* chain, const uint32_t* transition, double* out);
+int dhmc_generated_keyed_dev(dhmc_handle* h, const double* theta, int64_t n, int64_t first_problem, int64_t n_problems,
+                             const int64_t* chain, const uint32_t* transition, double* out);
 
 /* ---- state: initialization = (q, κ, ϵ), mcmc.jl:111-132 ---------------- */
 /* q: [D,B]; evaluates ℓ, ∇ℓ strictly (initialize_warmup_state, mcmc.jl:129-132). */
@@ -254,7 +270,11 @@ int dhmc_mcmc_dev(dhmc_handle* h, int32_t N, double* posterior, dhmc_tree_stats*
  * in place of D — the D parameters, then the G quantities g(θ) of every kept draw, with the same definitions (the shift
  * of the quantities' sums is g of the position the parameters' shift is).  reference, lo, hi [R, P], record [F, R, P],
  * counts [nbins + 2, R, P]; dhmc_summary_merge, dhmc_summary_finish and dhmc_histogram_quantiles take R as their row
- * count.  A non-finite g(θ) is folded as it is and sets no status bit.
+ * count.  A non-finite g(θ) is folded as it is and sets no status bit.  Random quantities (dhmc_generated_random) are
+ * ordinary rows: kept draw j of global chain g is evaluated under the key (seed, g) and t = t0 + (j + 1)·thin − 1, those
+ * of dhmc_generated_keyed; their shift is g of the shift position under the key (global id of the problem's first local
+ * chain, t0), which only keeps the sums free of cancellation.  Their reference cells are given by the caller (a NaN cell
+ * counts nothing: v < NaN is false); the arena grows by 2·P doubles for the shift's keys.
  *
  * The record is [DHMC_SUMMARY_FIELDS, D, P] column-major (the fields of (d, p) at (p·D + d)·F) and holds mergeable
  * quantities in absolute terms: the records of shards of one run (handles with different chain_offset, ranks) combine with

@@ -400,7 +400,9 @@ enum {
   DHMC_STREAM_PSEARCH = 1, /* momentum of the step-size search, mcmc.jl:138 */
   DHMC_STREAM_P = 2,       /* rand_p per transition, NUTS.jl:233 */
   DHMC_STREAM_DIR = 3,     /* Directions per transition, NUTS.jl:233 */
-  DHMC_STREAM_EXP = 4      /* randexp draws in merge order, NUTS.jl:44 */
+  DHMC_STREAM_EXP = 4,     /* randexp draws in merge order, NUTS.jl:44 */
+  DHMC_STREAM_GQ_U = 5,    /* uniforms of random generated quantities (dhmc_gq_uniform); the sampler never reads it */
+  DHMC_STREAM_GQ_N = 6     /* normals of random generated quantities (dhmc_gq_normal); the sampler never reads it */
 };
 
 typedef struct {
@@ -487,5 +489,17 @@ DHMC_HD double dm_randexp(dm_rng_key k, uint32_t t, uint32_t j) {
 DHMC_HD uint32_t dm_rand_directions(dm_rng_key k, uint32_t t) {
   return dm_rng_block(k, DHMC_STREAM_DIR, t, 0).v[0];
 }
+
+/* Random numbers of random generated quantities (include/dhmc_models.h, DHMC_USER_GENERATED_RNG): the key of one draw is
+ * (seed, global chain id) and the transition counter t of the transition that produced it.  uniform(i) and normal(i) are
+ * pure functions of (key, t, i): every quantity of a draw that asks for index i gets the same number, different indices
+ * are independent, uniforms and normals come from different streams (no shared bits), and neither stream is read by the
+ * sampler.  Host and device give the same bits. */
+typedef struct {
+  dm_rng_key key;
+  uint32_t t;
+} dhmc_gq_rng;
+DHMC_HD double dhmc_gq_uniform(const dhmc_gq_rng* r, uint32_t i) { return dm_uniform_elem(r->key, DHMC_STREAM_GQ_U, r->t, i); }
+DHMC_HD double dhmc_gq_normal(const dhmc_gq_rng* r, uint32_t i) { return dm_normal_elem(r->key, DHMC_STREAM_GQ_N, r->t, i); }
 
 #endif /* DHMC_MATH_H */

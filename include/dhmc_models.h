@@ -140,7 +140,29 @@ DHMC_HD double dhmc_logit_grad(double xtr, double beta) { return xtr - beta; }
  * them.  A non-finite value is folded as it is (NaN lands in the top histogram bin and is never below a reference) and
  * sets no chain status bit.  dhmc_generated evaluates them at given points; dhmc_mcmc_summary appends them to the
  * parameters as rows D … D + G − 1 (include/dhmc.h).  Where DHMC_USER_NGQ_CONST is defined as G, the bounds are checked
- * at compile time; otherwise dhmc_create checks G(D). */
+ * at compile time; otherwise dhmc_create checks G(D).
+ *
+ * Random generated quantities (optional, with DHMC_USER_GENERATED): Stan's `y_rep = normal_rng(...)`, e.g. posterior
+ * predictive replicates and the indicators of a posterior predictive check.  The quantity function takes a fifth argument:
+ *
+ *   #define DHMC_USER_GENERATED_RNG 1
+ *   DHMC_HD double dhmc_user_generated(int k, int D, const double* q, const double* params, const dhmc_gq_rng* rng);
+ *
+ * and draws its numbers through dhmc_math.h's two helpers, whose definitions are exact (the host reproduces them):
+ *   dhmc_gq_uniform(rng, i) = dm_uniform_elem(key, DHMC_STREAM_GQ_U, t, i)   in (0, 1)
+ *   dhmc_gq_normal(rng, i)  = dm_normal_elem(key, DHMC_STREAM_GQ_N, t, i)    N(0, 1)
+ * The numbers depend only on the key and the index i.  So every quantity of one draw sees the same normal(i), and a test
+ * statistic re-derives the replicate rows it summarizes by asking for the same indices (quantity k stays a pure function,
+ * evaluated independently of the others).  Different indices are independent; uniforms and normals never share bits; the
+ * sampler never reads either stream, so sampling is that of the same model without the part.  Other distributions are
+ * built by the header from these two: a Bernoulli(p) is uniform(i) < p; a Poisson by inversion over the indices i·64 + r,
+ * r = 0, 1, …; no further helper exists.
+ *
+ * The key of a kept draw: (the handle's seed, global chain id chain_offset + c) and t, the RNG counter of the transition
+ * that produced the draw.  A sampling call that starts at transition count t0 with thinning `thin` keeps, as draw j
+ * (0-based), the draw of t = t0 + (j + 1)·thin − 1 (uint32 arithmetic).  So, like the draws, the random quantities do
+ * not depend on sharding, chunking or checkpoint / restore.  dhmc_generated_keyed evaluates them at given points and
+ * keys; dhmc_generated refuses a model with random quantities. */
 #ifdef DHMC_USER_MODEL_HEADER
 #include DHMC_USER_MODEL_HEADER
 #ifndef DHMC_USER_NSUMS
@@ -163,6 +185,9 @@ DHMC_HD double dhmc_logit_grad(double xtr, double beta) { return xtr - beta; }
 #endif
 #if defined(DHMC_USER_NGQ_CONST) && !defined(DHMC_USER_GENERATED)
 #error "user model header: DHMC_USER_NGQ_CONST without DHMC_USER_GENERATED"
+#endif
+#if defined(DHMC_USER_GENERATED_RNG) && !defined(DHMC_USER_GENERATED)
+#error "user model header: DHMC_USER_GENERATED_RNG without DHMC_USER_GENERATED"
 #endif
 #define DHMC_HAVE_USER_FAMILY 1
 #endif

@@ -353,6 +353,27 @@ function generated(h::Handle, θ::AbstractArray{Float64}; n::Integer = size(θ, 
                  h.ptr, convert(Array{Float64}, θ), n, first_problem, n_problems, out))
     out
 end
+"1 when the handle's generated quantities are random (DHMC_USER_GENERATED_RNG; dhmc_generated_random), else 0."
+function generated_random(h::Handle)
+    r = Ref{Int32}(0)
+    _ck(h, ccall((:dhmc_generated_random, LIB), Cint, (Ptr{Cvoid}, Ptr{Int32}), h.ptr, r))
+    Int(r[])
+end
+"""`generated` with a key per point (dhmc_generated_keyed): point i of θ [D, n, n_problems] draws its random numbers under
+(the handle's seed, `chain[i]`) and `transition[i]`, each [n, n_problems].  Kept draw j (1-based) of chain k of a call
+that started at transition count t0 with thinning `thin` has chain = chain_offset + k − 1 and transition
+t0 + j·thin − 1.  A deterministic model ignores the keys."""
+function generated_keyed(h::Handle, θ::AbstractArray{Float64}, chain::AbstractArray{<:Integer},
+                         transition::AbstractArray{<:Integer}; n::Integer = size(θ, 2), first_problem::Integer = 0,
+                         n_problems::Integer = length(θ) ÷ (h.D * n))
+    G = generated_count(h)
+    out = Array{Float64}(undef, G, n, n_problems)
+    _ck(h, ccall((:dhmc_generated_keyed, LIB), Cint,
+                 (Ptr{Cvoid}, Ptr{Float64}, Int64, Int64, Int64, Ptr{Int64}, Ptr{UInt32}, Ptr{Float64}),
+                 h.ptr, convert(Array{Float64}, θ), n, first_problem, n_problems, convert(Array{Int64}, chain),
+                 convert(Array{UInt32}, transition), out))
+    out
+end
 """N transitions at the adapted (κ, ϵ), every `thin`-th folded on the device into per-(parameter, problem) statistics; no draw
 is returned.  `reference` [D, P] adds the SBC ranks.  Returns the mergeable record [SUMMARY_FIELDS, D, P] (merge shards with
 `summary_merge!`, finish with `summary_finish`).  A model with G generated quantities has D + G rows in place of D: the
