@@ -26,6 +26,7 @@
 #include <cmath>
 #include <cstdio>
 #include <fstream>
+#include <memory>
 #include <cstdlib>
 #include <cstring>
 #include <string>
@@ -312,6 +313,56 @@ __global__ void k_fill(double* dst, double v, size_t n) {
 }
 
 // ================================================================== host side
+#if defined(DHMC_ALLOC_FAULTS)
+// Fault-injection build (make faults, tests/test_device_allocations.py): the k-th next device allocation fails with
+// cudaErrorMemoryAllocation without reaching CUDA (k = 0: none fails), and the live allocations are counted.
+static int64_t g_fail_alloc_in = 0, g_live_allocations = 0;
+extern "C" void dhmc_test_fail_alloc(int64_t k) { g_fail_alloc_in = k; }
+extern "C" int64_t dhmc_test_live_allocations(void) { return g_live_allocations; }
+#endif
+
+// n elements of T in device memory, freed by the destructor; every device allocation of the host code is one of these.
+// alloc(n) frees the current array before it allocates, grow(n) allocates only for an n above the current size, and a
+// failed allocation leaves the array empty.
+template <class T>
+class DeviceArray {
+ public:
+  DeviceArray() = default;
+  DeviceArray(DeviceArray&& o) noexcept : p_(o.p_), n_(o.n_) { o.p_ = nullptr; o.n_ = 0; }
+  DeviceArray& operator=(DeviceArray&& o) noexcept {
+    if (this != &o) { reset(); std::swap(p_, o.p_); std::swap(n_, o.n_); }
+    return *this;
+  }
+  ~DeviceArray() { reset(); }
+  cudaError_t alloc(size_t n) {
+    reset();
+#if defined(DHMC_ALLOC_FAULTS)
+    if (g_fail_alloc_in > 0 && --g_fail_alloc_in == 0) return cudaErrorMemoryAllocation;
+#endif
+    const cudaError_t e = cudaMalloc(&p_, sizeof(T) * n);
+    if (e != cudaSuccess) { p_ = nullptr; return e; }
+    n_ = n;
+#if defined(DHMC_ALLOC_FAULTS)
+    if (p_) ++g_live_allocations;
+#endif
+    return cudaSuccess;
+  }
+  cudaError_t grow(size_t n) { return n > n_ ? alloc(n) : cudaSuccess; }
+  void reset() {
+#if defined(DHMC_ALLOC_FAULTS)
+    if (p_) --g_live_allocations;
+#endif
+    cudaFree(p_); p_ = nullptr; n_ = 0;
+  }
+  T* get() const { return p_; }
+  size_t size() const { return n_; }
+
+ private:
+  T* p_ = nullptr;
+  size_t n_ = 0;
+};
+
+// The handle owns its device arrays, events, streams, page-locked caller buffers and communicator.
 struct dhmc_handle {
   dhmc_config cfg;
   int T = 0, W = 0, EPL = 0;
@@ -320,59 +371,66 @@ struct dhmc_handle {
   size_t stride = 0;
   int n_slots = 0, n_sm = 0, grid = 0, sm_count = 0, light_grid = 0;
   int levels = 13, ntab = 64;       // stack entries per warp (max_depth + 1), slot-table entries (>= n_slots)
-  size_t smem_bytes = 0, smem_light = 0;
+  size_t smem_bytes = 0;
   size_t scratch_per_cta = 0;
+  bool planned = false;             // n_sm, smem_bytes, grid and scratch_per_cta match scratch and lr (plan)
   cudaStream_t stream = nullptr, copy_stream = nullptr, h2d_stream = nullptr;
   cudaEvent_t h2d_ev[16] = {};
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   cudaEvent_t chunk_ev[16] = {};
   cudaEvent_t copy_ev[16] = {};
   bool trace = false;
-  double* tmp_b = nullptr;          // [B] scratch (phase log densities) and [B·D] momentum override / [D·D] broadcast source,
-  double* tmp_bd = nullptr;         // allocated once instead of per call
-  unsigned* tmp_dir = nullptr;
-  size_t tmp_bd_doubles = 0;
+  DeviceArray<double> tmp_b;        // [B] scratch (phase log densities) and [B·D] momentum override / [D·D] broadcast source,
+  DeviceArray<double> tmp_bd;       // allocated once instead of per call
+  DeviceArray<unsigned> tmp_dir;
   std::vector<void*> registered;    // caller buffers page-locked on the fly (direct host writes of draws that exceed HBM)
-  void* stage[4] = {nullptr, nullptr, nullptr, nullptr};   // grow-only device staging for host outputs
-  size_t stage_bytes[4] = {0, 0, 0, 0};
-  double *q = nullptr, *g = nullptr, *lq = nullptr, *p = nullptr, *minv = nullptr, *eps = nullptr;
-  double* mparams = nullptr;
-  int* status = nullptr;
-  double* scratch = nullptr;
+  DeviceArray<char> stage[4];       // grow-only device staging for host outputs
+  DeviceArray<double> q, g, lq, p, minv, eps;
+  DeviceArray<double> mparams;
+  DeviceArray<int> status;
+  DeviceArray<double> scratch;
 #if defined(DHMC_PHASE_CLOCKS)
-  unsigned long long* phase_clocks = nullptr;   // leaf profile: kPhCount counters for each of up to 32 CTAs per SM
+  DeviceArray<unsigned long long> phase_clocks;   // leaf profile: kPhCount counters for each of up to 32 CTAs per SM
 #endif
-  unsigned* counter = nullptr;
-  unsigned long long* total_steps = nullptr;
+  DeviceArray<unsigned> counter;
+  DeviceArray<unsigned long long> total_steps;
   uint32_t t = 0;
   int64_t launches = 0;
   double last_ms = 0;
   int64_t last_steps = 0;
   bool has_position = false, has_eps = false;
   bool dense = false;               // κ is a Symmetric (dense) metric
-  double *minv_dense = nullptr, *wt = nullptr, *covt = nullptr, *dense_tmp = nullptr;
-  double* mean_pool = nullptr;      // pooled Symmetric stages: window mean of every chain [B][D]
+  DeviceArray<double> minv_dense, wt, covt, dense_tmp;
+  DeviceArray<double> mean_pool;    // pooled Symmetric stages: window mean of every chain [B][D]
   bool pooled = false;              // the dense metric is shared by every group of 8 chains
-  double* minv_pad = nullptr;       // packed groups on the tensor cores: zero-padded row blocks of every chain's M⁻¹
-  double *lX = nullptr, *lXt = nullptr, *ly = nullptr, *lr = nullptr;   // logistic regression
-  double* lXp = nullptr;            // … zero-padded row blocks of X for the tensor-core likelihood
+  DeviceArray<double> minv_pad;     // packed groups on the tensor cores: zero-padded row blocks of every chain's M⁻¹
+  DeviceArray<double> lX, lXt, ly, lr;   // logistic regression
+  DeviceArray<double> lXp;          // … zero-padded row blocks of X for the tensor-core likelihood
   int lN = 0, lLd = 0;              // (a batch: lN is the largest N, the row length of the residual scratch lr)
   // problem batch (dhmc_set_problems / _ragged): chains per problem (0 = one problem), problems, and the device table of
   // per-problem descriptors (where each problem's blocks start in mparams, lX, lXt, ly, lXp; its N and leading dimension)
   int64_t batch_k = 0, batch_p = 0;
-  ProblemDesc* problems = nullptr;
+  DeviceArray<ProblemDesc> problems;
   int reg_ctas[2] = {0, 0};         // occupancy of k_nuts (diag, dense)
   size_t smem_sm = 0, smem_cta_max = 0;
   ncclComm_t comm = nullptr;        // multi-GPU: one communicator per handle (dhmc_comm_init)
   int comm_nranks = 1, comm_rank = 0;
   double last_comm_ms = 0;
   // streaming summary (dhmc_mcmc_summary): grow-only device arena of the SummaryArgs arrays, and the struct itself
-  void* sum_buf = nullptr;
-  size_t sum_bytes = 0;
-  SummaryArgs* sum_args = nullptr;
+  DeviceArray<char> sum_buf;
+  DeviceArray<SummaryArgs> sum_args;
   int ngq = 0;                      // generated quantities of a user model (dhmc_generated_count)
   bool gq_random = false;           // ... drawn from the keyed streams (dhmc_generated_random)
   std::string err;
+
+  ~dhmc_handle() {                  // (the device arrays are freed after this body)
+    for (void* r : registered) cudaHostUnregister(r);
+    if (comm) dhmc_comm_destroy(this);
+    for (cudaEvent_t e : {ev0, ev1}) if (e) cudaEventDestroy(e);
+    for (cudaEvent_t* evs : {h2d_ev, chunk_ev, copy_ev})
+      for (int i = 0; i < 16; ++i) if (evs[i]) cudaEventDestroy(evs[i]);
+    for (cudaStream_t s : {copy_stream, h2d_stream, stream}) if (s) cudaStreamDestroy(s);
+  }
 };
 
 static std::string g_create_err;
@@ -388,7 +446,7 @@ static std::string g_create_err;
 
 // a per-chain staging vector in shared memory: mat-vec input (Symmetric metric), β (logistic), the whole position (USER)
 static bool needs_staging(const dhmc_handle* h) {
-  return h->minv_dense || h->cfg.family == DHMC_FAMILY_LOGISTIC || h->cfg.family == DHMC_FAMILY_USER;
+  return h->minv_dense.get() || h->cfg.family == DHMC_FAMILY_LOGISTIC || h->cfg.family == DHMC_FAMILY_USER;
 }
 // The instantiation of kernel k for the handle's family, layout and metric kind.  Part 3: the deep persistent kernels;
 // part 1: the persistent kernels of packed chain groups (the light kernels run one chain per CTA); part 0: the rest.
@@ -407,9 +465,9 @@ static size_t tma_rows(size_t n) { return (n + kTmaRows - 1) / kTmaRows * kTmaRo
 static int factor_grid(const dhmc_handle* h) { return (int)std::min<size_t>((size_t)h->sm_count * 4, (size_t)h->cfg.n_chains); }
 
 // rows of N doubles in the logistic scratch (residuals): one per CTA of the light kernels and, with one chain per CTA,
-// of the persistent kernels (packed groups keep theirs in shared memory)
-static size_t lr_rows(const dhmc_handle* h) {
-  return std::max<size_t>(h->G > 1 ? 0 : (size_t)h->grid, (size_t)h->light_grid);
+// of the persistent kernels of a plan of `grid` CTAs (packed groups keep theirs in shared memory)
+static size_t lr_rows(const dhmc_handle* h, int grid) {
+  return std::max<size_t>(h->G > 1 ? 0 : (size_t)grid, (size_t)h->light_grid);
 }
 
 // groups of the persistent kernels' reduction buffer (DeviceBackend::kFused): the last leaf of a depth-d adjacent tree carries
@@ -419,7 +477,8 @@ static int red_groups(const dhmc_handle* h) {
 }
 
 // Plan the persistent kernels for the current metric kind: CTAs per SM (register
-// limited), how many slots fit in shared memory, and the global scratch arena.
+// limited), how many slots fit in shared memory, and the global scratch arena.  The scratch of the current plan is freed
+// before the new one is allocated; if that allocation fails, the handle has no plan until the next successful one.
 static int plan(dhmc_handle* h) {
   const int T = h->T;
   const size_t B = (size_t)h->cfg.n_chains;
@@ -432,7 +491,6 @@ static int plan(dhmc_handle* h) {
                  : smem_layout(h->W, n_sm, slot_doubles, xs, h->levels, h->ntab, red_groups(h)).total;
   };
   struct { size_t total; } L0{heavy_smem(0)};
-  h->smem_light = smem_layout(h->W, 0, slot_doubles, xs).total;      // light kernels: standard layout
   int& reg_ctas = h->reg_ctas[h->dense ? 1 : 0];
   if (reg_ctas == 0) {
     const void* fn = handle_kernel(h, K_NUTS);
@@ -448,29 +506,17 @@ static int plan(dhmc_handle* h) {
   long n_sm = per_cta > L0.total ? (long)((per_cta - L0.total) / (slot_bytes * (size_t)G)) : 0;
   const int pool = h->n_slots - kWelfordSlots;   // the two highest slots stay in global memory
   if (n_sm > pool) n_sm = pool;
+  const int grid = (int)std::min<size_t>((size_t)ctas * h->sm_count, (B + G - 1) / G);
+  const size_t scratch_per_cta = (size_t)(h->n_slots - n_sm) * slot_doubles;
+  h->planned = false;
+  CK(h->scratch.alloc(scratch_per_cta * (size_t)grid * (size_t)G));
+  // (an access-policy window over the slot arena was tried and rejected: slower at C2)
+  if (h->lN) CK(h->lr.alloc((size_t)h->lN * lr_rows(h, grid)));   // residual scratch of the logistic family follows the grid
   h->n_sm = (int)n_sm;
   h->smem_bytes = heavy_smem(h->n_sm);
-  h->grid = (int)std::min<size_t>((size_t)ctas * h->sm_count, (B + G - 1) / G);
-  h->light_grid = (int)std::min<size_t>((size_t)h->sm_count * 16, B);
-  h->scratch_per_cta = (size_t)(h->n_slots - h->n_sm) * slot_doubles;
-  cudaFree(h->scratch); h->scratch = nullptr;
-  CK(cudaMalloc(&h->scratch, sizeof(double) * h->scratch_per_cta * (size_t)h->grid * (size_t)G));
-  // (an access-policy window over the slot arena was tried and rejected: slower at C2)
-  if (h->lN) {   // residual scratch of the logistic family follows the grid
-    cudaFree(h->lr); h->lr = nullptr;
-    CK(cudaMalloc(&h->lr, sizeof(double) * (size_t)h->lN * lr_rows(h)));
-  }
-  return DHMC_OK;
-}
-
-static int ensure_tmp(dhmc_handle* h, size_t doubles) {      // grow-only device scratch shared by the small entry points
-  if (!h->tmp_b) CK(cudaMalloc(&h->tmp_b, sizeof(double) * (size_t)h->cfg.n_chains));
-  if (!h->tmp_dir) CK(cudaMalloc(&h->tmp_dir, sizeof(unsigned) * (size_t)h->cfg.n_chains));
-  if (doubles > h->tmp_bd_doubles) {
-    cudaFree(h->tmp_bd); h->tmp_bd = nullptr; h->tmp_bd_doubles = 0;
-    CK(cudaMalloc(&h->tmp_bd, sizeof(double) * doubles));
-    h->tmp_bd_doubles = doubles;
-  }
+  h->grid = grid;
+  h->scratch_per_cta = scratch_per_cta;
+  h->planned = true;
   return DHMC_OK;
 }
 
@@ -479,23 +525,23 @@ static KArgs base_args(dhmc_handle* h) {
   std::memset(&a, 0, sizeof(a));
   a.D = (int)h->cfg.dim; a.B = (int)h->cfg.n_chains; a.T = h->T; a.W = h->W;
   a.seed = h->cfg.seed; a.chain_offset = h->cfg.chain_offset;
-  a.q = h->q; a.g = h->g; a.lq = h->lq; a.p = h->p; a.minv = h->minv; a.eps = h->eps;
-  a.mparams = h->mparams; a.status = h->status;
+  a.q = h->q.get(); a.g = h->g.get(); a.lq = h->lq.get(); a.p = h->p.get(); a.minv = h->minv.get(); a.eps = h->eps.get();
+  a.mparams = h->mparams.get(); a.status = h->status.get();
   a.max_depth = h->cfg.max_depth; a.min_delta = h->cfg.min_delta;
   a.t0 = h->t;
-  a.scratch = h->scratch; a.scratch_per_cta = h->scratch_per_cta;
+  a.scratch = h->scratch.get(); a.scratch_per_cta = h->scratch_per_cta;
 #if defined(DHMC_PHASE_CLOCKS)
-  a.phase_clocks = h->phase_clocks;
+  a.phase_clocks = h->phase_clocks.get();
 #endif
   a.n_sm = h->n_sm; a.n_slots = h->n_slots; a.stride = h->stride * (h->dense ? 2 : 1);
   a.levels = h->levels; a.ntab = h->ntab;
   a.red_groups = red_groups(h);
-  a.counter = h->counter; a.total_steps = h->total_steps;
+  a.counter = h->counter.get(); a.total_steps = h->total_steps.get();
   a.chain_begin = 0; a.chain_end = (int)h->cfg.n_chains;
-  a.minv_dense = h->minv_dense; a.wt = h->wt; a.covt = nullptr; a.minv_pad = h->minv_pad; a.mean_out = nullptr; a.pooled = h->pooled ? 1 : 0;
+  a.minv_dense = h->minv_dense.get(); a.wt = h->wt.get(); a.covt = nullptr; a.minv_pad = h->minv_pad.get(); a.mean_out = nullptr; a.pooled = h->pooled;
   a.xs_doubles = needs_staging(h) ? (int)((size_t)h->T * h->EPL) : 0;
-  a.lX = h->lX; a.lXt = h->lXt; a.ly = h->ly; a.lr = h->lr; a.lN = h->lN; a.lLd = h->lLd; a.lXp = h->lXp;
-  a.batch_k = (int)h->batch_k; a.problems = h->problems;
+  a.lX = h->lX.get(); a.lXt = h->lXt.get(); a.ly = h->ly.get(); a.lr = h->lr.get(); a.lN = h->lN; a.lLd = h->lLd; a.lXp = h->lXp.get();
+  a.batch_k = (int)h->batch_k; a.problems = h->problems.get();
   return a;
 }
 
@@ -511,14 +557,16 @@ static int read_timer(dhmc_handle* h) {
 // before and right after the kernel, so that they time it alone.  reset_steps: zero the Σ steps counter first.
 static int launch(dhmc_handle* h, KernelId k, KArgs a, cudaEvent_t before, cudaEvent_t after, bool reset_steps = true) {
   const bool heavy = (k == K_NUTS || k == K_SEARCH);
+  if (!h->planned) { h->err = "the handle has no kernel plan: its re-plan failed to allocate the slot scratch; set the metric "
+                             "again (dhmc_set_metric, dhmc_set_metric_dense) to re-plan"; return DHMC_ENOMEM; }
   if (!heavy) { a.n_sm = 0; a.red_groups = 1; }
   const size_t smem = heavy ? h->smem_bytes : smem_layout(h->W, 0, a.stride, (size_t)a.xs_doubles).total;
   int grid = heavy ? h->grid : h->light_grid;
   const int G = heavy ? h->G : 1;
   if (heavy) grid = std::max(1, std::min(grid, (a.chain_end - a.chain_begin + G - 1) / G));
   if (heavy) {
-    CK(cudaMemsetAsync(h->counter, 0, sizeof(unsigned), h->stream));
-    if (reset_steps) CK(cudaMemsetAsync(h->total_steps, 0, sizeof(unsigned long long), h->stream));
+    CK(cudaMemsetAsync(h->counter.get(), 0, sizeof(unsigned), h->stream));
+    if (reset_steps) CK(cudaMemsetAsync(h->total_steps.get(), 0, sizeof(unsigned long long), h->stream));
   }
   if (before) CK(cudaEventRecord(before, h->stream));
   {
@@ -539,7 +587,7 @@ static int sync_and_check_status(dhmc_handle* h, int mask, const char* what) {
   CK(cudaStreamSynchronize(h->stream));
   const size_t B = (size_t)h->cfg.n_chains;
   std::vector<int> st(B);
-  CK(cudaMemcpy(st.data(), h->status, sizeof(int) * B, cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(st.data(), h->status.get(), sizeof(int) * B, cudaMemcpyDeviceToHost));
   long bad = 0, first = -1, halted = 0, first_halted = -1;
   for (size_t i = 0; i < B; ++i) {
     if (st[i] & mask) { if (first < 0) first = (long)i; ++bad; }
@@ -592,33 +640,59 @@ static void choose_layout(int64_t D, int req_T, int* T, int* EPL) {
 extern "C" {
 
 const char* dhmc_last_error(dhmc_handle* h) { return h ? h->err.c_str() : g_create_err.c_str(); }
-int dhmc_comm_destroy(dhmc_handle* h);
 
 int dhmc_destroy(dhmc_handle* h) {
   if (!h) return DHMC_OK;
   cudaSetDevice(h->cfg.device);
-  cudaFree(h->q); cudaFree(h->g); cudaFree(h->lq); cudaFree(h->p); cudaFree(h->minv); cudaFree(h->eps);
-  cudaFree(h->mparams); cudaFree(h->status); cudaFree(h->scratch); cudaFree(h->counter);
-#if defined(DHMC_PHASE_CLOCKS)
-  cudaFree(h->phase_clocks);
-#endif
-  cudaFree(h->total_steps);
-  cudaFree(h->minv_dense); cudaFree(h->wt); cudaFree(h->covt); cudaFree(h->dense_tmp); cudaFree(h->minv_pad); cudaFree(h->mean_pool);
-  cudaFree(h->lX); cudaFree(h->lXt); cudaFree(h->ly); cudaFree(h->lr); cudaFree(h->lXp); cudaFree(h->problems);
-  cudaFree(h->tmp_b); cudaFree(h->tmp_bd); cudaFree(h->tmp_dir);
-  cudaFree(h->sum_buf); cudaFree(h->sum_args);
-  for (void* r : h->registered) cudaHostUnregister(r);
-  if (h->comm) dhmc_comm_destroy(h);
-  if (h->ev0) cudaEventDestroy(h->ev0);
-  if (h->ev1) cudaEventDestroy(h->ev1);
-  for (auto& e : h->chunk_ev) if (e) cudaEventDestroy(e);
-  for (auto& e : h->copy_ev) if (e) cudaEventDestroy(e);
-  for (auto& b : h->stage) cudaFree(b);
-  if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
-  for (auto& e : h->h2d_ev) if (e) cudaEventDestroy(e);
-  if (h->h2d_stream) cudaStreamDestroy(h->h2d_stream);
-  if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
+  return DHMC_OK;
+}
+
+// dhmc_create after its argument checks: the device resources of the new handle and its first plan
+static int init_handle(dhmc_handle* h, const dhmc_config* cfg) {
+  CK(cudaSetDevice(cfg->device));
+  cudaDeviceProp prop;
+  CK(cudaGetDeviceProperties(&prop, cfg->device));
+  h->sm_count = prop.multiProcessorCount;
+#if defined(DHMC_PHASE_CLOCKS)
+  CK(h->phase_clocks.alloc((size_t)kPhCount * 32 * (size_t)h->sm_count));
+  CK(cudaMemset(h->phase_clocks.get(), 0, sizeof(unsigned long long) * kPhCount * 32 * (size_t)h->sm_count));
+#endif
+  CK(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
+  CK(cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking));
+  CK(cudaStreamCreateWithFlags(&h->h2d_stream, cudaStreamNonBlocking));
+  const bool trace = std::getenv("DHMC_TRACE") != nullptr;      // DHMC_TRACE=1: timeline of the chunk pipeline on stderr
+  for (cudaEvent_t* evs : {h->h2d_ev, h->chunk_ev, h->copy_ev})
+    for (int i = 0; i < 16; ++i) CK(cudaEventCreateWithFlags(&evs[i], trace ? cudaEventDefault : cudaEventDisableTiming));
+  h->trace = trace;
+  CK(cudaEventCreate(&h->ev0));
+  CK(cudaEventCreate(&h->ev1));
+  const size_t B = (size_t)cfg->n_chains, D = (size_t)cfg->dim;
+  CK(h->q.alloc(B * D));
+  CK(h->g.alloc(B * D));
+  CK(h->p.alloc(B * D));
+  CK(h->minv.alloc(B * D));
+  CK(h->lq.alloc(B));
+  CK(h->eps.alloc(B));
+  CK(h->status.alloc(B));
+  CK(h->counter.alloc(1));
+  CK(h->total_steps.alloc(1));
+  CK(h->mparams.alloc(2 * D));
+  CK(cudaMemsetAsync(h->q.get(), 0, sizeof(double) * B * D, h->stream));
+  CK(cudaMemsetAsync(h->g.get(), 0, sizeof(double) * B * D, h->stream));
+  CK(cudaMemsetAsync(h->p.get(), 0, sizeof(double) * B * D, h->stream));
+  CK(cudaMemsetAsync(h->lq.get(), 0, sizeof(double) * B, h->stream));
+  CK(cudaMemsetAsync(h->eps.get(), 0, sizeof(double) * B, h->stream));
+  CK(cudaMemsetAsync(h->status.get(), 0, sizeof(int) * B, h->stream));
+  CK(cudaMemsetAsync(h->mparams.get(), 0, sizeof(double) * 2 * D, h->stream));
+  k_fill<<<1024, 256, 0, h->stream>>>(h->minv.get(), 1.0, B * D);   // κ = GaussianKineticEnergy(D), mcmc.jl:130
+  h->launches += 1;
+
+  h->smem_sm = (size_t)prop.sharedMemPerMultiprocessor;          // 228 KB
+  h->smem_cta_max = (size_t)prop.sharedMemPerBlockOptin;         // 227 KB
+  h->light_grid = (int)std::min<size_t>((size_t)h->sm_count * 16, B);
+  if (int rc = plan(h)) return rc;
+  CK(cudaStreamSynchronize(h->stream));
   return DHMC_OK;
 }
 
@@ -667,63 +741,15 @@ int dhmc_create(const dhmc_config* cfg, dhmc_handle** out) {
     return DHMC_ECUDA;
   }
   if (cfg->device < 0 || cfg->device >= ndev) { g_create_err = "bad device ordinal"; return DHMC_EARG; }
-  dhmc_handle* h = new dhmc_handle();
+  std::unique_ptr<dhmc_handle> h(new dhmc_handle());
   h->cfg = *cfg; h->T = T; h->W = T / 32; h->EPL = EPL; h->stride = (size_t)T * EPL; h->G = pack; h->deep = deep;
   h->ngq = ngq;
   h->gq_random = ngq > 0 && dhmc_user_family_random && dhmc_user_family_random() != 0;
   h->n_slots = slots_needed(cfg->max_depth);
   h->levels = deep ? cfg->max_depth + 1 : kStdLevels;        // deep persistent kernels size their stack / slot table at run time
   h->ntab = deep ? std::max(kStdTab, (h->n_slots + 7) & ~7) : kStdTab;
-  auto fail = [&](int rc) { g_create_err = h->err; dhmc_destroy(h); return rc; };
-#define CKC(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { h->err = std::string(#call) + ": " + cudaGetErrorString(e_); return fail(e_ == cudaErrorMemoryAllocation ? DHMC_ENOMEM : DHMC_ECUDA); } } while (0)
-  CKC(cudaSetDevice(cfg->device));
-  cudaDeviceProp prop;
-  CKC(cudaGetDeviceProperties(&prop, cfg->device));
-  h->sm_count = prop.multiProcessorCount;
-#if defined(DHMC_PHASE_CLOCKS)
-  CKC(cudaMalloc(&h->phase_clocks, sizeof(unsigned long long) * kPhCount * 32 * (size_t)h->sm_count));
-  CKC(cudaMemset(h->phase_clocks, 0, sizeof(unsigned long long) * kPhCount * 32 * (size_t)h->sm_count));
-#endif
-  CKC(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-  CKC(cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking));
-  CKC(cudaStreamCreateWithFlags(&h->h2d_stream, cudaStreamNonBlocking));
-  const bool trace = std::getenv("DHMC_TRACE") != nullptr;      // DHMC_TRACE=1: timeline of the chunk pipeline on stderr
-  for (auto& e : h->h2d_ev) CKC(cudaEventCreateWithFlags(&e, trace ? cudaEventDefault : cudaEventDisableTiming));
-  for (auto& e : h->chunk_ev) CKC(cudaEventCreateWithFlags(&e, trace ? cudaEventDefault : cudaEventDisableTiming));
-  for (auto& e : h->copy_ev) CKC(cudaEventCreateWithFlags(&e, trace ? cudaEventDefault : cudaEventDisableTiming));
-  h->trace = trace;
-  CKC(cudaEventCreate(&h->ev0));
-  CKC(cudaEventCreate(&h->ev1));
-  const size_t B = (size_t)cfg->n_chains, D = (size_t)cfg->dim;
-  CKC(cudaMalloc(&h->q, sizeof(double) * B * D));
-  CKC(cudaMalloc(&h->g, sizeof(double) * B * D));
-  CKC(cudaMalloc(&h->p, sizeof(double) * B * D));
-  CKC(cudaMalloc(&h->minv, sizeof(double) * B * D));
-  CKC(cudaMalloc(&h->lq, sizeof(double) * B));
-  CKC(cudaMalloc(&h->eps, sizeof(double) * B));
-  CKC(cudaMalloc(&h->status, sizeof(int) * B));
-  CKC(cudaMalloc(&h->counter, sizeof(unsigned)));
-  CKC(cudaMalloc(&h->total_steps, sizeof(unsigned long long)));
-  CKC(cudaMalloc(&h->mparams, sizeof(double) * 2 * D));
-  CKC(cudaMemsetAsync(h->q, 0, sizeof(double) * B * D, h->stream));
-  CKC(cudaMemsetAsync(h->g, 0, sizeof(double) * B * D, h->stream));
-  CKC(cudaMemsetAsync(h->p, 0, sizeof(double) * B * D, h->stream));
-  CKC(cudaMemsetAsync(h->lq, 0, sizeof(double) * B, h->stream));
-  CKC(cudaMemsetAsync(h->eps, 0, sizeof(double) * B, h->stream));
-  CKC(cudaMemsetAsync(h->status, 0, sizeof(int) * B, h->stream));
-  CKC(cudaMemsetAsync(h->mparams, 0, sizeof(double) * 2 * D, h->stream));
-  k_fill<<<1024, 256, 0, h->stream>>>(h->minv, 1.0, B * D);   // κ = GaussianKineticEnergy(D), mcmc.jl:130
-  h->launches += 1;
-
-  h->smem_sm = (size_t)prop.sharedMemPerMultiprocessor;          // 228 KB
-  h->smem_cta_max = (size_t)prop.sharedMemPerBlockOptin;         // 227 KB
-  {
-    int rcp = plan(h);
-    if (rcp != DHMC_OK) return fail(rcp);
-  }
-  CKC(cudaStreamSynchronize(h->stream));
-#undef CKC
-  *out = h;
+  if (int rc = init_handle(h.get(), cfg)) { g_create_err = h->err; return rc; }
+  *out = h.release();
   return DHMC_OK;
 }
 
@@ -816,51 +842,49 @@ static int install_problems(dhmc_handle* h, const double* params, const std::vec
   }
   CK(cudaSetDevice(h->cfg.device));
   CK(cudaStreamSynchronize(h->stream));
-  double *mp = nullptr, *X = nullptr, *Xt = nullptr, *y = nullptr, *Xp = nullptr, *lr = nullptr;
-  ProblemDesc* dd = nullptr;
-  auto drop = [&] { cudaFree(mp); cudaFree(X); cudaFree(Xt); cudaFree(y); cudaFree(Xp); cudaFree(lr); cudaFree(dd); };
-#define CKB(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { h->err = std::string(#call) + ": " + cudaGetErrorString(e_); \
-    cudaStreamSynchronize(h->stream); drop(); return e_ == cudaErrorMemoryAllocation ? DHMC_ENOMEM : DHMC_ECUDA; } } while (0)
-  if (K) {
-    CKB(cudaMalloc(&dd, sizeof(ProblemDesc) * Pz));
-    CKB(cudaMemcpyAsync(dd, desc.data(), sizeof(ProblemDesc) * Pz, cudaMemcpyHostToDevice, h->stream));
-  }
-  if (fam == DHMC_FAMILY_LOGISTIC) {
-    // per problem: X [N][D], Xᵀ [D][ld], y [N] and, for packed groups, the zero-padded row blocks [rows][xs]; one residual
-    // scratch of rows of the largest N
-    CKB(cudaMalloc(&X, sizeof(double) * tX));
-    CKB(cudaMalloc(&Xt, sizeof(double) * tXt));
-    CKB(cudaMalloc(&y, sizeof(double) * ty));
-    CKB(cudaMalloc(&lr, sizeof(double) * maxN * lr_rows(h)));
-    if (h->G > 1) CKB(cudaMalloc(&Xp, sizeof(double) * tXp));
-    for (size_t p = 0; p < Pz; ++p) {
-      const double* blk = params + offs[p];
-      const ProblemDesc& d = desc[p];
-      const size_t N = (size_t)d.N;
-      CKB(cudaMemcpyAsync(X + d.X, blk + 1, sizeof(double) * N * D, cudaMemcpyHostToDevice, h->stream));
-      CKB(cudaMemcpyAsync(y + d.y, blk + 1 + N * D, sizeof(double) * N, cudaMemcpyHostToDevice, h->stream));
-      k_transpose<<<1024, 256, 0, h->stream>>>(X + d.X, Xt + d.Xt, N, D, (size_t)d.ld);
-      if (Xp) k_pad_rows<<<1024, 256, 0, h->stream>>>(X + d.X, Xp + d.Xp, N, D, tma_rows(N), xs, 1);
-      h->launches += Xp ? 2 : 1;
+  DeviceArray<double> mp, X, Xt, y, Xp, lr;
+  DeviceArray<ProblemDesc> dd;
+  const int rc = [&]() -> int {
+    if (K) {
+      CK(dd.alloc(Pz));
+      CK(cudaMemcpyAsync(dd.get(), desc.data(), sizeof(ProblemDesc) * Pz, cudaMemcpyHostToDevice, h->stream));
     }
-  } else if (fam == DHMC_FAMILY_DIAG_NORMAL || fam == DHMC_FAMILY_USER) {   // (STD_NORMAL and FUNNEL have no parameters)
-    // mparams is never null, also for a USER model without parameters
-    CKB(cudaMalloc(&mp, sizeof(double) * std::max<size_t>(offs[Pz], 1)));
-    if (offs[Pz]) CKB(cudaMemcpyAsync(mp, params, sizeof(double) * offs[Pz], cudaMemcpyHostToDevice, h->stream));
-  }
-  CKB(cudaGetLastError());
-  CKB(cudaStreamSynchronize(h->stream));
-#undef CKB
+    if (fam == DHMC_FAMILY_LOGISTIC) {
+      // per problem: X [N][D], Xᵀ [D][ld], y [N] and, for packed groups, the zero-padded row blocks [rows][xs]; one residual
+      // scratch of rows of the largest N
+      CK(X.alloc(tX));
+      CK(Xt.alloc(tXt));
+      CK(y.alloc(ty));
+      CK(lr.alloc(maxN * lr_rows(h, h->grid)));
+      if (h->G > 1) CK(Xp.alloc(tXp));
+      for (size_t p = 0; p < Pz; ++p) {
+        const double* blk = params + offs[p];
+        const ProblemDesc& d = desc[p];
+        const size_t N = (size_t)d.N;
+        CK(cudaMemcpyAsync(X.get() + d.X, blk + 1, sizeof(double) * N * D, cudaMemcpyHostToDevice, h->stream));
+        CK(cudaMemcpyAsync(y.get() + d.y, blk + 1 + N * D, sizeof(double) * N, cudaMemcpyHostToDevice, h->stream));
+        k_transpose<<<1024, 256, 0, h->stream>>>(X.get() + d.X, Xt.get() + d.Xt, N, D, (size_t)d.ld);
+        if (Xp.get()) k_pad_rows<<<1024, 256, 0, h->stream>>>(X.get() + d.X, Xp.get() + d.Xp, N, D, tma_rows(N), xs, 1);
+        h->launches += Xp.get() ? 2 : 1;
+      }
+    } else if (fam == DHMC_FAMILY_DIAG_NORMAL || fam == DHMC_FAMILY_USER) {   // (STD_NORMAL and FUNNEL have no parameters)
+      // mparams is never null, also for a USER model without parameters
+      CK(mp.alloc(std::max<size_t>(offs[Pz], 1)));
+      if (offs[Pz]) CK(cudaMemcpyAsync(mp.get(), params, sizeof(double) * offs[Pz], cudaMemcpyHostToDevice, h->stream));
+    }
+    CK(cudaGetLastError());
+    return DHMC_OK;
+  }();
+  // the new arrays are freed on an error only after the copies and kernels queued on them
+  if (rc != DHMC_OK) { cudaStreamSynchronize(h->stream); return rc; }
+  CK(cudaStreamSynchronize(h->stream));
   if (fam == DHMC_FAMILY_LOGISTIC) {
-    cudaFree(h->lX); cudaFree(h->lXt); cudaFree(h->ly); cudaFree(h->lr); cudaFree(h->lXp);
-    h->lX = X; h->lXt = Xt; h->ly = y; h->lr = lr; h->lXp = Xp;
+    h->lX = std::move(X); h->lXt = std::move(Xt); h->ly = std::move(y); h->lr = std::move(lr); h->lXp = std::move(Xp);
     h->lN = (int)maxN; h->lLd = desc[0].ld;    // a chain's own N and ld come from its descriptor
-  } else if (mp) {
-    cudaFree(h->mparams);
-    h->mparams = mp;
+  } else if (mp.get()) {
+    h->mparams = std::move(mp);
   }
-  cudaFree(h->problems);
-  h->problems = dd;
+  h->problems = std::move(dd);
   h->batch_k = K; h->batch_p = K ? P : 0;
   return DHMC_OK;
 }
@@ -901,7 +925,7 @@ int dhmc_set_problems_ragged(dhmc_handle* h, const double* params, const size_t*
 }
 
 static int eval_position(dhmc_handle* h, bool randomize) {
-  CK(cudaMemsetAsync(h->status, 0, sizeof(int) * (size_t)h->cfg.n_chains, h->stream));
+  CK(cudaMemsetAsync(h->status.get(), 0, sizeof(int) * (size_t)h->cfg.n_chains, h->stream));
   KArgs a = base_args(h);
   a.strict = 1; a.randomize = randomize ? 1 : 0;
   int rc = launch(h, K_EVAL, a, nullptr, nullptr);
@@ -913,7 +937,7 @@ static int eval_position(dhmc_handle* h, bool randomize) {
 int dhmc_set_position(dhmc_handle* h, const double* q) {
   if (!h || !q) return DHMC_EARG;
   CK(cudaSetDevice(h->cfg.device));
-  CK(cudaMemcpyAsync(h->q, q, sizeof(double) * (size_t)h->cfg.n_chains * h->cfg.dim, cudaMemcpyHostToDevice, h->stream));
+  CK(cudaMemcpyAsync(h->q.get(), q, sizeof(double) * (size_t)h->cfg.n_chains * h->cfg.dim, cudaMemcpyHostToDevice, h->stream));
   return eval_position(h, false);
 }
 int dhmc_random_position(dhmc_handle* h) {
@@ -922,37 +946,43 @@ int dhmc_random_position(dhmc_handle* h) {
   return eval_position(h, true);
 }
 
+// The arrays of the Symmetric metric, allocated together at the first use.  A handle without a plan re-plans here too.
 static int ensure_dense(dhmc_handle* h) {
-  if (h->minv_dense) return DHMC_OK;
-
+  if (h->minv_dense.get()) return h->planned ? DHMC_OK : plan(h);
   const size_t B = (size_t)h->cfg.n_chains, dd = (size_t)h->cfg.dim * h->cfg.dim;
-  CK(cudaMalloc(&h->minv_dense, sizeof(double) * B * dd));
-  CK(cudaMalloc(&h->wt, sizeof(double) * B * dd));
-  CK(cudaMalloc(&h->covt, sizeof(double) * B * dd));
-  CK(cudaMalloc(&h->dense_tmp, sizeof(double) * 3 * dd * (size_t)factor_grid(h)));
-  CK(cudaMemsetAsync(h->wt, 0, sizeof(double) * B * dd, h->stream));
+  DeviceArray<double> minv_dense, wt, covt, dense_tmp, minv_pad;
+  CK(minv_dense.alloc(B * dd));
+  CK(wt.alloc(B * dd));
+  CK(covt.alloc(B * dd));
+  CK(dense_tmp.alloc(3 * dd * (size_t)factor_grid(h)));
   if (h->G > 1)     // [B][⌈D/32⌉·32][XS]: one bulk copy per 32-row block (coop_matvec_tma)
-    CK(cudaMalloc(&h->minv_pad, sizeof(double) * B * tma_rows((size_t)h->cfg.dim) * (size_t)tma_xs((int)h->cfg.dim)));
+    CK(minv_pad.alloc(B * tma_rows((size_t)h->cfg.dim) * (size_t)tma_xs((int)h->cfg.dim)));
+  h->minv_dense = std::move(minv_dense); h->wt = std::move(wt); h->covt = std::move(covt);
+  h->dense_tmp = std::move(dense_tmp); h->minv_pad = std::move(minv_pad);
+  CK(cudaMemsetAsync(h->wt.get(), 0, sizeof(double) * B * dd, h->stream));
   // re-planned whatever the metric kind: with the dense arrays allocated, the shared-memory layout carries the staging
   // vector (needs_staging) also for the diagonal kernels
   return plan(h);
 }
-// The metric kind of the handle's kernels: the persistent kernels are re-planned when the slot width (dense) changes.
+// The metric kind of the handle's kernels: the persistent kernels are re-planned when the slot width (dense) changes, or
+// when the handle has no plan.  The kind changes only with a successful plan.
 static int set_metric_kind(dhmc_handle* h, bool dense, bool pooled) {
-  h->pooled = pooled;
-  if (h->dense == dense) return DHMC_OK;
+  if (h->planned && h->dense == dense) { h->pooled = pooled; return DHMC_OK; }
+  const bool was_dense = h->dense;
   h->dense = dense;
-  return plan(h);
+  if (int rc = plan(h)) { h->dense = was_dense; return rc; }
+  h->pooled = pooled;
+  return DHMC_OK;
 }
 // κ = GaussianKineticEnergy(Symmetric M⁻¹): W = cholesky(inv(M⁻¹)).L on device, then switch
 // the handle to the dense kernels (pooled: M⁻¹ is shared by every group of 8 chains).
 static int factor_and_switch(dhmc_handle* h, bool pooled) {
   const size_t B = (size_t)h->cfg.n_chains, D = (size_t)h->cfg.dim;
-  CK(cudaMemsetAsync(h->status, 0, sizeof(int) * B, h->stream));
-  k_dense_factor<<<factor_grid(h), 128, 0, h->stream>>>(h->minv_dense, h->wt, h->dense_tmp, h->status, (int)D, (int)B);
+  CK(cudaMemsetAsync(h->status.get(), 0, sizeof(int) * B, h->stream));
+  k_dense_factor<<<factor_grid(h), 128, 0, h->stream>>>(h->minv_dense.get(), h->wt.get(), h->dense_tmp.get(), h->status.get(), (int)D, (int)B);
   h->launches += 1;
-  if (h->minv_pad) {
-    k_pad_rows<<<2048, 256, 0, h->stream>>>(h->minv_dense, h->minv_pad, D, D, tma_rows(D), (size_t)tma_xs((int)D), B);
+  if (h->minv_pad.get()) {
+    k_pad_rows<<<2048, 256, 0, h->stream>>>(h->minv_dense.get(), h->minv_pad.get(), D, D, tma_rows(D), (size_t)tma_xs((int)D), B);
     h->launches += 1;
   }
   CK(cudaGetLastError());
@@ -967,14 +997,13 @@ int dhmc_set_metric_dense(dhmc_handle* h, const double* minv, int broadcast) {
   if (rc != DHMC_OK) return rc;
   const size_t B = (size_t)h->cfg.n_chains, dd = (size_t)h->cfg.dim * h->cfg.dim;
   if (broadcast) {
-    int rct = ensure_tmp(h, dd);
-    if (rct != DHMC_OK) return rct;
-    CK(cudaMemcpyAsync(h->tmp_bd, minv, sizeof(double) * dd, cudaMemcpyHostToDevice, h->stream));
-    k_broadcast<<<1024, 256, 0, h->stream>>>(h->minv_dense, h->tmp_bd, dd, B);
+    CK(h->tmp_bd.grow(dd));
+    CK(cudaMemcpyAsync(h->tmp_bd.get(), minv, sizeof(double) * dd, cudaMemcpyHostToDevice, h->stream));
+    k_broadcast<<<1024, 256, 0, h->stream>>>(h->minv_dense.get(), h->tmp_bd.get(), dd, B);
     h->launches += 1;
     CK(cudaStreamSynchronize(h->stream));
   } else {
-    CK(cudaMemcpyAsync(h->minv_dense, minv, sizeof(double) * B * dd, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(h->minv_dense.get(), minv, sizeof(double) * B * dd, cudaMemcpyHostToDevice, h->stream));
   }
   return factor_and_switch(h, false);
 }
@@ -982,7 +1011,7 @@ int dhmc_get_metric_dense(dhmc_handle* h, double* minv) {
   if (!h || !minv) return DHMC_EARG;
   if (!h->dense) { h->err = "the current metric is diagonal"; return DHMC_EARG; }
   CK(cudaSetDevice(h->cfg.device));
-  CK(cudaMemcpy(minv, h->minv_dense, sizeof(double) * (size_t)h->cfg.n_chains * h->cfg.dim * h->cfg.dim, cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(minv, h->minv_dense.get(), sizeof(double) * (size_t)h->cfg.n_chains * h->cfg.dim * h->cfg.dim, cudaMemcpyDeviceToHost));
   return DHMC_OK;
 }
 int dhmc_metric_is_dense(dhmc_handle* h, int32_t* dense) { if (!h || !dense) return DHMC_EARG; *dense = h->dense ? 1 : 0; return DHMC_OK; }
@@ -992,15 +1021,14 @@ int dhmc_set_metric(dhmc_handle* h, const double* minv, int broadcast) {
   CK(cudaSetDevice(h->cfg.device));
   const size_t B = (size_t)h->cfg.n_chains, D = (size_t)h->cfg.dim;
   if (!minv) {
-    k_fill<<<1024, 256, 0, h->stream>>>(h->minv, 1.0, B * D);
+    k_fill<<<1024, 256, 0, h->stream>>>(h->minv.get(), 1.0, B * D);
   } else if (broadcast) {
-    int rct = ensure_tmp(h, D);
-    if (rct != DHMC_OK) return rct;
-    CK(cudaMemcpyAsync(h->tmp_bd, minv, sizeof(double) * D, cudaMemcpyHostToDevice, h->stream));
-    k_broadcast<<<1024, 256, 0, h->stream>>>(h->minv, h->tmp_bd, D, B);
+    CK(h->tmp_bd.grow(D));
+    CK(cudaMemcpyAsync(h->tmp_bd.get(), minv, sizeof(double) * D, cudaMemcpyHostToDevice, h->stream));
+    k_broadcast<<<1024, 256, 0, h->stream>>>(h->minv.get(), h->tmp_bd.get(), D, B);
     CK(cudaStreamSynchronize(h->stream));
   } else {
-    CK(cudaMemcpyAsync(h->minv, minv, sizeof(double) * B * D, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(h->minv.get(), minv, sizeof(double) * B * D, cudaMemcpyHostToDevice, h->stream));
   }
   h->launches += 1;
   CK(cudaStreamSynchronize(h->stream));
@@ -1013,11 +1041,11 @@ int dhmc_set_stepsize(dhmc_handle* h, const double* eps, int broadcast) {
   const size_t B = (size_t)h->cfg.n_chains;
   if (broadcast) {
     if (!(eps[0] > 0)) { h->err = "ϵ > 0"; return DHMC_EARG; }    // stepsize.jl:135
-    k_fill<<<256, 256, 0, h->stream>>>(h->eps, eps[0], B);
+    k_fill<<<256, 256, 0, h->stream>>>(h->eps.get(), eps[0], B);
     h->launches += 1;
   } else {
     for (size_t i = 0; i < B; ++i) if (!(eps[i] > 0)) { h->err = "ϵ > 0"; return DHMC_EARG; }
-    CK(cudaMemcpyAsync(h->eps, eps, sizeof(double) * B, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(h->eps.get(), eps, sizeof(double) * B, cudaMemcpyHostToDevice, h->stream));
   }
   CK(cudaStreamSynchronize(h->stream));
   h->has_eps = true;
@@ -1027,7 +1055,7 @@ int dhmc_set_stepsize(dhmc_handle* h, const double* eps, int broadcast) {
 int dhmc_set_momentum(dhmc_handle* h, const double* p) {
   if (!h || !p) return DHMC_EARG;
   CK(cudaSetDevice(h->cfg.device));
-  CK(cudaMemcpyAsync(h->p, p, sizeof(double) * (size_t)h->cfg.n_chains * h->cfg.dim, cudaMemcpyHostToDevice, h->stream));
+  CK(cudaMemcpyAsync(h->p.get(), p, sizeof(double) * (size_t)h->cfg.n_chains * h->cfg.dim, cudaMemcpyHostToDevice, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   return DHMC_OK;
 }
@@ -1036,12 +1064,12 @@ int dhmc_get_state(dhmc_handle* h, double* q, double* lq, double* grad, double* 
   if (!h) return DHMC_EARG;
   CK(cudaSetDevice(h->cfg.device));
   const size_t B = (size_t)h->cfg.n_chains, D = (size_t)h->cfg.dim;
-  if (q) CK(cudaMemcpyAsync(q, h->q, sizeof(double) * B * D, cudaMemcpyDeviceToHost, h->stream));
-  if (grad) CK(cudaMemcpyAsync(grad, h->g, sizeof(double) * B * D, cudaMemcpyDeviceToHost, h->stream));
-  if (minv) CK(cudaMemcpyAsync(minv, h->minv, sizeof(double) * B * D, cudaMemcpyDeviceToHost, h->stream));
-  if (p) CK(cudaMemcpyAsync(p, h->p, sizeof(double) * B * D, cudaMemcpyDeviceToHost, h->stream));
-  if (lq) CK(cudaMemcpyAsync(lq, h->lq, sizeof(double) * B, cudaMemcpyDeviceToHost, h->stream));
-  if (eps) CK(cudaMemcpyAsync(eps, h->eps, sizeof(double) * B, cudaMemcpyDeviceToHost, h->stream));
+  if (q) CK(cudaMemcpyAsync(q, h->q.get(), sizeof(double) * B * D, cudaMemcpyDeviceToHost, h->stream));
+  if (grad) CK(cudaMemcpyAsync(grad, h->g.get(), sizeof(double) * B * D, cudaMemcpyDeviceToHost, h->stream));
+  if (minv) CK(cudaMemcpyAsync(minv, h->minv.get(), sizeof(double) * B * D, cudaMemcpyDeviceToHost, h->stream));
+  if (p) CK(cudaMemcpyAsync(p, h->p.get(), sizeof(double) * B * D, cudaMemcpyDeviceToHost, h->stream));
+  if (lq) CK(cudaMemcpyAsync(lq, h->lq.get(), sizeof(double) * B, cudaMemcpyDeviceToHost, h->stream));
+  if (eps) CK(cudaMemcpyAsync(eps, h->eps.get(), sizeof(double) * B, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   return DHMC_OK;
 }
@@ -1049,7 +1077,7 @@ int dhmc_get_state(dhmc_handle* h, double* q, double* lq, double* grad, double* 
 int dhmc_chain_status(dhmc_handle* h, int32_t* status) {
   if (!h || !status) return DHMC_EARG;
   CK(cudaSetDevice(h->cfg.device));
-  CK(cudaMemcpy(status, h->status, sizeof(int) * (size_t)h->cfg.n_chains, cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(status, h->status.get(), sizeof(int) * (size_t)h->cfg.n_chains, cudaMemcpyDeviceToHost));
   return DHMC_OK;
 }
 int dhmc_get_transition_count(dhmc_handle* h, uint32_t* t) { if (!h || !t) return DHMC_EARG; *t = h->t; return DHMC_OK; }
@@ -1059,7 +1087,7 @@ int dhmc_leapfrog(dhmc_handle* h, int32_t n_steps, int32_t sign) {
   if (!h || n_steps < 0) return DHMC_EARG;
   if (!h->has_position || !h->has_eps) { h->err = "dhmc_leapfrog: set position and step size first"; return DHMC_EARG; }
   CK(cudaSetDevice(h->cfg.device));
-  CK(cudaMemsetAsync(h->status, 0, sizeof(int) * (size_t)h->cfg.n_chains, h->stream));   // status words describe the current call
+  CK(cudaMemsetAsync(h->status.get(), 0, sizeof(int) * (size_t)h->cfg.n_chains, h->stream));   // status words describe the current call
   KArgs a = base_args(h);
   a.lf_steps = n_steps; a.lf_sign = sign;
   int rc = launch(h, K_LEAPFROG, a, h->ev0, h->ev1);
@@ -1073,13 +1101,12 @@ int dhmc_phase_logdensity(dhmc_handle* h, double* out) {
   if (!h || !out) return DHMC_EARG;
   CK(cudaSetDevice(h->cfg.device));
   const size_t B = (size_t)h->cfg.n_chains;
-  int rc = ensure_tmp(h, 0);
-  if (rc != DHMC_OK) return rc;
+  CK(h->tmp_b.grow(B));
   KArgs a = base_args(h);
-  a.out_phase = h->tmp_b;
-  rc = launch(h, K_PHASE, a, nullptr, nullptr);
+  a.out_phase = h->tmp_b.get();
+  const int rc = launch(h, K_PHASE, a, nullptr, nullptr);
   if (rc != DHMC_OK) return rc;
-  CK(cudaMemcpyAsync(out, h->tmp_b, sizeof(double) * B, cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaMemcpyAsync(out, h->tmp_b.get(), sizeof(double) * B, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   return DHMC_OK;
 }
@@ -1093,7 +1120,7 @@ int dhmc_find_initial_stepsize(dhmc_handle* h, double initial_eps, double log_th
   if (!h->has_position) { h->err = "set the position first"; return DHMC_EARG; }
   if (h->has_eps) { h->err = "stepsize ϵ manually specified, won't perform initial search"; return DHMC_EARG; }  // mcmc.jl:137
   CK(cudaSetDevice(h->cfg.device));
-  CK(cudaMemsetAsync(h->status, 0, sizeof(int) * (size_t)h->cfg.n_chains, h->stream));   // status words describe the current call
+  CK(cudaMemsetAsync(h->status.get(), 0, sizeof(int) * (size_t)h->cfg.n_chains, h->stream));   // status words describe the current call
   KArgs a = base_args(h);
   a.s_init = initial_eps; a.s_thresh = log_threshold; a.s_maxiter = maxiter;
   int rc = launch(h, K_SEARCH, a, h->ev0, h->ev1);
@@ -1111,13 +1138,6 @@ int dhmc_find_initial_stepsize(dhmc_handle* h, double initial_eps, double log_th
 // chunk is one k_nuts launch on the compute stream, and its draws/statistics are
 // copied D2H on the copy stream while the next chunk computes (pinned host
 // buffers make the copies truly asynchronous; pageable ones still work).
-static int ensure_stage(dhmc_handle* h, int i, size_t bytes) {
-  if (h->stage_bytes[i] >= bytes) return DHMC_OK;
-  cudaFree(h->stage[i]); h->stage[i] = nullptr; h->stage_bytes[i] = 0;
-  CK(cudaMalloc(&h->stage[i], bytes));
-  h->stage_bytes[i] = bytes;
-  return DHMC_OK;
-}
 // Is `p` page-locked host memory that the device can address (cudaHostAlloc / cudaHostRegister)?  Then *dev is its device alias.
 static bool host_mapped(const void* p, void** dev) {
   const char* evn = std::getenv("DHMC_NO_DIRECT");        // A/B switch: always stage
@@ -1161,7 +1181,7 @@ static int run_nuts(dhmc_handle* h, int N, const AdaptConfig& cfg, double lambda
       // kernel writes the host buffer directly when they do not fit (DHMC_DIRECT=1 forces it).
       size_t fr = 0, tot = 0;
       cudaMemGetInfo(&fr, &tot);
-      const bool fits = bytes <= h->stage_bytes[0] || bytes + ((size_t)1 << 30) <= fr;
+      const bool fits = bytes <= h->stage[0].size() || bytes + ((size_t)1 << 30) <= fr;
       const char* evd = std::getenv("DHMC_DIRECT");
       const bool force_direct = evd && std::atoi(evd) == 1;
       if (!fits || force_direct) {
@@ -1179,19 +1199,18 @@ static int run_nuts(dhmc_handle* h, int N, const AdaptConfig& cfg, double lambda
       o.direct = host_mapped(o.host, &o.dev);
     }
     if (!o.direct) {
-      if ((rc = ensure_stage(h, i, bytes)) != DHMC_OK) return rc;
-      o.dev = h->stage[i];
+      CK(h->stage[i].grow(bytes));
+      o.dev = h->stage[i].get();
     }
   }
-  if (p_over_host || dir_over_host) {
-    if ((rc = ensure_tmp(h, p_over_host ? B * D : 0)) != DHMC_OK) return rc;
-  }
   if (p_over_host) {
-    d_p = h->tmp_bd;
+    CK(h->tmp_bd.grow(B * D));
+    d_p = h->tmp_bd.get();
     CK(cudaMemcpyAsync(d_p, p_over_host, sizeof(double) * B * D, cudaMemcpyHostToDevice, h->stream));
   }
   if (dir_over_host) {
-    d_dir = h->tmp_dir;
+    CK(h->tmp_dir.grow(B));
+    d_dir = h->tmp_dir.get();
     CK(cudaMemcpyAsync(d_dir, dir_over_host, sizeof(unsigned) * B, cudaMemcpyHostToDevice, h->stream));
   }
   tr_pt[0] = tr_ms();
@@ -1199,8 +1218,8 @@ static int run_nuts(dhmc_handle* h, int N, const AdaptConfig& cfg, double lambda
   a.N = N; a.thin = thin; a.N_keep = (int)n; a.cfg = cfg; a.p_override = d_p; a.dir_override = d_dir;
   a.out_q = (double*)out[0].dev; a.out_stats = (dhmc_tree_stats*)out[1].dev; a.out_eps = (double*)out[2].dev;
   a.out_lq = (double*)out[3].dev;
-  if (cfg.metric == DHMC_METRIC_SYMMETRIC) a.covt = h->covt;
-  if (pool_metric) a.mean_out = h->mean_pool;
+  if (cfg.metric == DHMC_METRIC_SYMMETRIC) a.covt = h->covt.get();
+  if (pool_metric) a.mean_out = h->mean_pool.get();
   a.summary = summary;
   const size_t out_bytes = posterior ? sizeof(double) * B * n * D : 0;
   // chunks must stay many waves long, or the ragged tail of every chunk idles the SMs
@@ -1210,7 +1229,7 @@ static int run_nuts(dhmc_handle* h, int N, const AdaptConfig& cfg, double lambda
   int nchunks = (!outputs_on_device && B >= 4096 && (staged_big || q_host)) ? 16 : 1;
   while (nchunks > 1 && B / (size_t)nchunks < (size_t)8 * (size_t)h->grid * (size_t)h->G) nchunks /= 2;   // >= 8 waves of chain slots per chunk
   if (const char* ev = std::getenv("DHMC_E2E_CHUNKS")) { const int v = std::atoi(ev); if (v >= 1 && v <= 16 && !outputs_on_device) nchunks = v; }
-  CK(cudaMemsetAsync(h->status, 0, sizeof(int) * B, h->stream));   // status words describe the current call
+  CK(cudaMemsetAsync(h->status.get(), 0, sizeof(int) * B, h->stream));   // status words describe the current call
   for (int ci = 0; ci < nchunks; ++ci) {
     // (a pooled metric, and a batch on packed groups, keep their groups of 8 chains inside one chunk)
     const size_t unit = (h->pooled || (h->G > 1 && h->batch_k)) ? 8 : 1;
@@ -1224,7 +1243,7 @@ static int run_nuts(dhmc_handle* h, int N, const AdaptConfig& cfg, double lambda
         CK(cudaEventRecord(h->h2d_ev[15], h->stream));
         CK(cudaStreamWaitEvent(h->h2d_stream, h->h2d_ev[15], 0));
       }
-      CK(cudaMemcpyAsync(h->q + c0 * D, q_host + c0 * D, sizeof(double) * nc * D, cudaMemcpyHostToDevice, h->h2d_stream));
+      CK(cudaMemcpyAsync(h->q.get() + c0 * D, q_host + c0 * D, sizeof(double) * nc * D, cudaMemcpyHostToDevice, h->h2d_stream));
       CK(cudaEventRecord(h->h2d_ev[ci], h->h2d_stream));
       CK(cudaStreamWaitEvent(h->stream, h->h2d_ev[ci], 0));
       KArgs ea = a;
@@ -1248,7 +1267,7 @@ static int run_nuts(dhmc_handle* h, int N, const AdaptConfig& cfg, double lambda
   }
   tr_pt[1] = tr_ms();
   unsigned long long steps = 0;
-  CK(cudaMemcpyAsync(&steps, h->total_steps, sizeof steps, cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaMemcpyAsync(&steps, h->total_steps.get(), sizeof steps, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   tr_pt[2] = tr_ms();
   CK(cudaStreamSynchronize(h->copy_stream));
@@ -1284,9 +1303,9 @@ static int run_nuts(dhmc_handle* h, int N, const AdaptConfig& cfg, double lambda
     // κ = GaussianKineticEnergy(regularize_M⁻¹(sample_M⁻¹(Symmetric, X), λ)) — mcmc.jl:282
     const int fgrid = factor_grid(h);
     if (pool_metric)
-      k_cov_pool<<<fgrid, 128, sizeof(double) * h->cfg.dim, h->stream>>>(h->covt, h->mean_pool, h->minv_dense, N, lambda, (int)h->cfg.dim, (int)h->cfg.n_chains);
+      k_cov_pool<<<fgrid, 128, sizeof(double) * h->cfg.dim, h->stream>>>(h->covt.get(), h->mean_pool.get(), h->minv_dense.get(), N, lambda, (int)h->cfg.dim, (int)h->cfg.n_chains);
     else
-      k_cov_finish<<<fgrid, 128, 0, h->stream>>>(h->covt, h->minv_dense, N, lambda, (int)h->cfg.dim, (int)h->cfg.n_chains);
+      k_cov_finish<<<fgrid, 128, 0, h->stream>>>(h->covt.get(), h->minv_dense.get(), N, lambda, (int)h->cfg.dim, (int)h->cfg.n_chains);
     h->launches += 1;
     rc = factor_and_switch(h, pool_metric);
   }
@@ -1321,7 +1340,7 @@ int dhmc_warmup_stage(dhmc_handle* h, int32_t N, int32_t metric, const dhmc_dual
     cfg.adapt = 1; cfg.delta = da->delta; cfg.gamma = da->gamma; cfg.kappa = da->kappa; cfg.t0 = da->t0;
   }
   if (cfg.metric == DHMC_METRIC_SYMMETRIC) { int rcd = ensure_dense(h); if (rcd != DHMC_OK) return rcd; }
-  if (pool && !h->mean_pool) CK(cudaMalloc(&h->mean_pool, sizeof(double) * (size_t)h->cfg.n_chains * (size_t)h->cfg.dim));
+  if (pool) CK(h->mean_pool.grow((size_t)h->cfg.n_chains * (size_t)h->cfg.dim));
   return run_nuts(h, N, cfg, lambda, nullptr, nullptr, posterior, stats, eps_used, logdens, false, true, nullptr, 1, pool);
 }
 
@@ -1427,8 +1446,8 @@ static int launch_generated(dhmc_handle* h, const double* theta, int64_t n, int6
                             const uint32_t* transition, double* out) {
   const int64_t pts = n * n_problems;
   const int grid = (int)std::min<int64_t>(pts, (int64_t)h->sm_count * 16);
-  const int e = dhmc_user_family_generated(theta, n, n_problems, (int)h->cfg.dim, h->ngq, h->mparams,
-                                           h->batch_k ? h->problems : nullptr, first, (const long long*)chain, transition,
+  const int e = dhmc_user_family_generated(theta, n, n_problems, (int)h->cfg.dim, h->ngq, h->mparams.get(),
+                                           h->batch_k ? h->problems.get() : nullptr, first, (const long long*)chain, transition,
                                            (unsigned long long)h->cfg.seed, out, h->T, grid, h->stream);
   if (e != cudaSuccess) { h->err = std::string("k_generated: ") + cudaGetErrorString((cudaError_t)e); return DHMC_ECUDA; }
   h->launches += 1;
@@ -1505,20 +1524,19 @@ static int generated_host(dhmc_handle* h, const double* theta, int64_t n, int64_
       if (chain[i] < 0 || chain[i] >= ((int64_t)1 << 56)) { h->err = "dhmc_generated_keyed: chain ids lie in [0, 2^56)"; return DHMC_EARG; }
   CK(cudaSetDevice(h->cfg.device));
   // one buffer: points [pts][D], out [pts][G], then with keys chain [pts] (8-byte) and transition [pts] (4-byte)
-  double* buf = nullptr;
-  CK(cudaMalloc(&buf, sizeof(double) * pts * (D + G) + (keyed ? (sizeof(int64_t) + sizeof(uint32_t)) * pts : 0)));
-  int64_t* dchain = keyed ? (int64_t*)(buf + pts * (D + G)) : nullptr;
+  DeviceArray<char> buf;
+  CK(buf.alloc(sizeof(double) * pts * (D + G) + (keyed ? (sizeof(int64_t) + sizeof(uint32_t)) * pts : 0)));
+  double* dtheta = (double*)buf.get();
+  double* dout = dtheta + pts * D;
+  int64_t* dchain = keyed ? (int64_t*)(dout + pts * G) : nullptr;
   uint32_t* dtrans = keyed ? (uint32_t*)(dchain + pts) : nullptr;
-  cudaError_t e = cudaMemcpyAsync(buf, theta, sizeof(double) * pts * D, cudaMemcpyHostToDevice, h->stream);
-  if (keyed && e == cudaSuccess) e = cudaMemcpyAsync(dchain, chain, sizeof(int64_t) * pts, cudaMemcpyHostToDevice, h->stream);
-  if (keyed && e == cudaSuccess) e = cudaMemcpyAsync(dtrans, transition, sizeof(uint32_t) * pts, cudaMemcpyHostToDevice, h->stream);
-  int rg = e == cudaSuccess ? launch_generated(h, buf, n, first, n_problems, dchain, dtrans, buf + pts * D) : DHMC_OK;
-  if (e == cudaSuccess && rg == DHMC_OK)
-    e = cudaMemcpyAsync(out, buf + pts * D, sizeof(double) * pts * G, cudaMemcpyDeviceToHost, h->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
-  cudaFree(buf);
-  if (e != cudaSuccess) { h->err = std::string("dhmc_generated: ") + cudaGetErrorString(e); return DHMC_ECUDA; }
-  return rg;
+  CK(cudaMemcpyAsync(dtheta, theta, sizeof(double) * pts * D, cudaMemcpyHostToDevice, h->stream));
+  if (keyed) CK(cudaMemcpyAsync(dchain, chain, sizeof(int64_t) * pts, cudaMemcpyHostToDevice, h->stream));
+  if (keyed) CK(cudaMemcpyAsync(dtrans, transition, sizeof(uint32_t) * pts, cudaMemcpyHostToDevice, h->stream));
+  if (int rg = launch_generated(h, dtheta, n, first, n_problems, dchain, dtrans, dout)) return rg;
+  CK(cudaMemcpyAsync(out, dout, sizeof(double) * pts * G, cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  return DHMC_OK;
 }
 
 int dhmc_generated_dev(dhmc_handle* h, const double* theta, int64_t n, int64_t first_problem, int64_t n_problems, double* out) {
@@ -1558,26 +1576,30 @@ static int mcmc_summary(dhmc_handle* h, int32_t N, int32_t thin, const double* r
   // arrays of SummaryArgs' g-fields, laid out as the parameters' with ng in place of D
   const size_t ng = (size_t)h->ngq, R = D + ng, PG = P * ng, grows = (size_t)h->grid * h->G * 5 * ng;
   const size_t gstage = (size_t)h->grid * h->G * cells * ng;
-  // one grow-only arena: acc [P][5][D], shift [P][D], ref [P][D], row [grid·G][3][D], below [P][D], chains [P], then with
-  // histograms hist [P][D][cells], lo [P][D], inv_w [P][D]; the same for the generated quantities (gacc, gshift, gref, grow,
-  // gbelow, ghist, glo, ginv_w; 8-byte elements); last stage [grid·G][cells][D] and gstage [grid·G][cells][ng] (4-byte)
-  // random generated quantities: last the keys of the shift's points, chain [P] (8-byte) and transition [P] (4-byte), 8-aligned
-  const size_t body = sizeof(double) * (8 * PD + rows + P + PD * cells + (counts ? 2 * PD : 0)) + sizeof(unsigned) * stage +
-                      sizeof(double) * (8 * PG + grows + PG * cells + (counts ? 2 * PG : 0)) + sizeof(unsigned) * gstage;
-  const size_t keys_at = (body + 7) & ~(size_t)7;
-  const size_t need = h->gq_random ? keys_at + (sizeof(int64_t) + sizeof(uint32_t)) * P : body;
-  if (need > h->sum_bytes) {
-    cudaFree(h->sum_buf); h->sum_buf = nullptr; h->sum_bytes = 0;
-    CK(cudaMalloc(&h->sum_buf, need));
-    h->sum_bytes = need;
-  }
-  if (!h->sum_args) CK(cudaMalloc(&h->sum_args, sizeof(SummaryArgs)));
-  double* acc = (double*)h->sum_buf;
-  double* shift = acc + 5 * PD;
-  double* ref = shift + PD;
-  double* row = ref + PD;
-  unsigned long long* below = (unsigned long long*)(row + rows);
-  unsigned long long* chains = below + PD;
+  // one grow-only arena of the arrays below, in this order (8-byte elements, then the 4-byte staging rows, then the 8-aligned
+  // keys of random generated quantities): carve(nullptr) measures it, carve(base) places the arrays in it
+  double *acc, *shift, *ref, *row, *lo = nullptr, *inv_w = nullptr, *gacc, *gshift, *gref, *grow, *glo = nullptr, *ginv_w = nullptr;
+  unsigned long long *below, *chains, *hist, *gbelow, *ghist;
+  unsigned *stg, *gstg;                        // histogram staging rows [grid·G][cells][D], [grid·G][cells][ng]
+  int64_t* kchain = nullptr;                   // keys of the shift's points, chain [P] and transition [P]
+  uint32_t* ktrans = nullptr;
+  auto carve = [&](char* base) {
+    size_t at = 0;
+    auto take = [&](auto& ptr, size_t n) {
+      ptr = base ? reinterpret_cast<std::remove_reference_t<decltype(ptr)>>(base + at) : nullptr;
+      at += sizeof(*ptr) * n;
+    };
+    take(acc, 5 * PD); take(shift, PD); take(ref, PD); take(row, rows); take(below, PD); take(chains, P); take(hist, PD * cells);
+    if (counts) { take(lo, PD); take(inv_w, PD); }
+    take(gacc, 5 * PG); take(gshift, PG); take(gref, PG); take(grow, grows); take(gbelow, PG); take(ghist, PG * cells);
+    if (counts) { take(glo, PG); take(ginv_w, PG); }
+    take(stg, stage); take(gstg, gstage);
+    if (h->gq_random) { at = (at + 7) & ~(size_t)7; take(kchain, P); take(ktrans, P); }
+    return at;
+  };
+  CK(h->sum_buf.grow(carve(nullptr)));
+  carve(h->sum_buf.get());
+  CK(h->sum_args.grow(1));
   CK(cudaMemsetAsync(acc, 0, sizeof(double) * 5 * PD, h->stream));
   CK(cudaMemsetAsync(below, 0, sizeof(unsigned long long) * (PD + P), h->stream));
   if (reference) CK(upload_rows(ref, reference, 0, D, R, P, h->stream));
@@ -1585,41 +1607,27 @@ static int mcmc_summary(dhmc_handle* h, int32_t N, int32_t thin, const double* r
   // the first, those chains are K apart: one strided copy (a first problem entered in its middle takes one more).
   const int64_t p0 = K ? off / K : 0, p1 = K ? (off + (int64_t)B - 1) / K : 0;
   const int64_t pa = (K && off % K) ? p0 + 1 : p0;
-  if (pa > p0) CK(cudaMemcpyAsync(shift + p0 * D, h->q, sizeof(double) * D, cudaMemcpyDeviceToDevice, h->stream));
+  if (pa > p0) CK(cudaMemcpyAsync(shift + p0 * D, h->q.get(), sizeof(double) * D, cudaMemcpyDeviceToDevice, h->stream));
   if (p1 >= pa)
-    CK(cudaMemcpy2DAsync(shift + pa * D, sizeof(double) * D, h->q + (size_t)(K ? pa * K - off : 0) * D, sizeof(double) * D * (size_t)(K ? K : 1),
+    CK(cudaMemcpy2DAsync(shift + pa * D, sizeof(double) * D, h->q.get() + (size_t)(K ? pa * K - off : 0) * D, sizeof(double) * D * (size_t)(K ? K : 1),
                          sizeof(double) * D, (size_t)(p1 - pa + 1), cudaMemcpyDeviceToDevice, h->stream));
   SummaryArgs sa{row, shift, reference ? ref : nullptr, acc, below, chains, n_keep / 2, nullptr, nullptr, nullptr, nullptr, 0};
-  unsigned long long* hist = chains + P;
-  double* lo = (double*)(hist + PD * cells);
-  double* inv_w = lo + PD;
-  double* gacc = counts ? inv_w + PD : (double*)hist;
   std::vector<double> hinv(counts ? P * R : 0);
   for (size_t i = 0; i < hinv.size(); ++i) hinv[i] = (double)nbins / (hi_host[i] - lo_host[i]);
   if (counts) {
     CK(cudaMemsetAsync(hist, 0, sizeof(unsigned long long) * PD * cells, h->stream));
     CK(upload_rows(lo, lo_host, 0, D, R, P, h->stream));
     CK(upload_rows(inv_w, hinv.data(), 0, D, R, P, h->stream));
-    sa.lo = lo; sa.inv_w = inv_w; sa.stage = (unsigned*)(gacc + 8 * PG + grows + PG * cells + 2 * PG); sa.hist = hist; sa.nbins = nbins;
+    sa.lo = lo; sa.inv_w = inv_w; sa.stage = stg; sa.hist = hist; sa.nbins = nbins;
   }
-  // generated quantities: gacc [P][5][ng], gshift, gref [P][ng], grow [grid·G][5][ng], gbelow [P][ng], then with histograms
-  // ghist [P][ng][cells], glo, ginv_w [P][ng]; the shift is g(shift), evaluated on the device
-  double* gshift = gacc + 5 * PG;
-  double* gref = gshift + PG;
-  double* grow = gref + PG;
-  unsigned long long* gbelow = (unsigned long long*)(grow + grows);
-  unsigned long long* ghist = gbelow + PG;
+  // generated quantities: the shift is g(shift), evaluated on the device
   if (ng) {
     CK(cudaMemsetAsync(gacc, 0, sizeof(double) * 5 * PG, h->stream));
     CK(cudaMemsetAsync(gbelow, 0, sizeof(unsigned long long) * PG, h->stream));
     // random quantities: the shift's key is (global id of the problem's first local chain, the call's first transition);
     // it only sets the cancellation shift of the sums
-    int64_t* kchain = nullptr;
-    uint32_t* ktrans = nullptr;
     if (h->gq_random) {
       const size_t np = (size_t)(p1 - p0 + 1);
-      kchain = (int64_t*)((char*)h->sum_buf + keys_at);
-      ktrans = (uint32_t*)(kchain + np);
       std::vector<int64_t> hc(np);
       std::vector<uint32_t> ht(np, h->t);
       for (size_t i = 0; i < np; ++i) hc[i] = K ? std::max((p0 + (int64_t)i) * K, off) : off;
@@ -1629,22 +1637,20 @@ static int mcmc_summary(dhmc_handle* h, int32_t N, int32_t thin, const double* r
     const int rg = launch_generated(h, shift + p0 * D, 1, p0, p1 - p0 + 1, kchain, ktrans, gshift + p0 * ng);
     if (rg != DHMC_OK) return rg;
     if (reference) CK(upload_rows(gref, reference, D, ng, R, P, h->stream));
-    sa.ng = (int)ng; sa.mparams = h->mparams; sa.problems = K ? h->problems : nullptr;
+    sa.ng = (int)ng; sa.mparams = h->mparams.get(); sa.problems = K ? h->problems.get() : nullptr;
     sa.seed = (unsigned long long)h->cfg.seed; sa.chain_offset = (long long)off; sa.t0 = h->t; sa.thin = thin;
     sa.grow = grow; sa.gshift = gshift; sa.gref = reference ? gref : nullptr; sa.gacc = gacc; sa.gbelow = gbelow;
     if (counts) {
-      double* glo = (double*)(ghist + PG * cells);
-      double* ginv_w = glo + PG;
       CK(cudaMemsetAsync(ghist, 0, sizeof(unsigned long long) * PG * cells, h->stream));
       CK(upload_rows(glo, lo_host, D, ng, R, P, h->stream));
       CK(upload_rows(ginv_w, hinv.data(), D, ng, R, P, h->stream));
-      sa.glo = glo; sa.ginv_w = ginv_w; sa.gstage = sa.stage + stage; sa.ghist = ghist;
+      sa.glo = glo; sa.ginv_w = ginv_w; sa.gstage = gstg; sa.ghist = ghist;
     }
   }
-  CK(cudaMemcpyAsync(h->sum_args, &sa, sizeof sa, cudaMemcpyHostToDevice, h->stream));
+  CK(cudaMemcpyAsync(h->sum_args.get(), &sa, sizeof sa, cudaMemcpyHostToDevice, h->stream));
   AdaptConfig cfg{};
   const int rc = run_nuts(h, N, cfg, 0.0, nullptr, nullptr, nullptr, stats, nullptr, logdens, false, true, nullptr, thin, false,
-                          h->sum_args);
+                          h->sum_args.get());
   if (rc != DHMC_OK && rc != DHMC_ENUMERIC) return rc;    // a chain that failed is left out of its problem's sums
   std::vector<double> hacc(5 * PD), hshift(PD), hgacc(5 * PG), hgshift(PG);
   std::vector<unsigned long long> hcnt(PD + P), hgcnt(PG);
@@ -1652,7 +1658,7 @@ static int mcmc_summary(dhmc_handle* h, int32_t N, int32_t thin, const double* r
   CK(cudaMemcpyAsync(hshift.data(), shift, sizeof(double) * PD, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaMemcpyAsync(hcnt.data(), below, sizeof(unsigned long long) * hcnt.size(), cudaMemcpyDeviceToHost, h->stream));
   // [P][D][cells] is the column-major [cells, D, P] of the ABI; uint64 counts stay far below 2^63
-  if (counts && !ng) CK(cudaMemcpyAsync(counts, below + PD + P, sizeof(int64_t) * PD * cells, cudaMemcpyDeviceToHost, h->stream));
+  if (counts && !ng) CK(cudaMemcpyAsync(counts, hist, sizeof(int64_t) * PD * cells, cudaMemcpyDeviceToHost, h->stream));
   if (ng) {            // counts [cells, R, P]: the D parameter rows, then the ng generated rows of each problem
     CK(cudaMemcpyAsync(hgacc.data(), gacc, sizeof(double) * hgacc.size(), cudaMemcpyDeviceToHost, h->stream));
     CK(cudaMemcpyAsync(hgshift.data(), gshift, sizeof(double) * PG, cudaMemcpyDeviceToHost, h->stream));
@@ -1828,22 +1834,20 @@ int dhmc_tree_summary_dev(dhmc_handle* h, const dhmc_tree_stats* stats_dev, int3
   if (!h || !stats_dev || N < 1) return DHMC_EARG;
   CK(cudaSetDevice(h->cfg.device));
   const int B = (int)h->cfg.n_chains;
-  unsigned long long* d_cnt = nullptr;   // [33 depth][3 term][1 steps]
-  double* d_f = nullptr;                 // [1 acc][B ebfmi]
-  CK(cudaMalloc(&d_cnt, sizeof(unsigned long long) * 37));
-  CK(cudaMalloc(&d_f, sizeof(double) * (1 + (size_t)B)));
-  CK(cudaMemsetAsync(d_cnt, 0, sizeof(unsigned long long) * 37, h->stream));
-  CK(cudaMemsetAsync(d_f, 0, sizeof(double), h->stream));
-  k_tree_summary<<<h->sm_count * 8, 256, 0, h->stream>>>(stats_dev, N, B, d_cnt, d_cnt + 33, d_f, d_cnt + 36, ebfmi ? d_f + 1 : nullptr);
+  DeviceArray<unsigned long long> d_cnt;   // [33 depth][3 term][1 steps]
+  DeviceArray<double> d_f;                 // [1 acc][B ebfmi]
+  CK(d_cnt.alloc(37));
+  CK(d_f.alloc(1 + (size_t)B));
+  CK(cudaMemsetAsync(d_cnt.get(), 0, sizeof(unsigned long long) * 37, h->stream));
+  CK(cudaMemsetAsync(d_f.get(), 0, sizeof(double), h->stream));
+  k_tree_summary<<<h->sm_count * 8, 256, 0, h->stream>>>(stats_dev, N, B, d_cnt.get(), d_cnt.get() + 33, d_f.get(), d_cnt.get() + 36, ebfmi ? d_f.get() + 1 : nullptr);
   h->launches += 1;
   unsigned long long cnt[37];
   double acc = 0;
-  cudaError_t e = cudaMemcpyAsync(cnt, d_cnt, sizeof cnt, cudaMemcpyDeviceToHost, h->stream);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(&acc, d_f, sizeof acc, cudaMemcpyDeviceToHost, h->stream);
-  if (e == cudaSuccess && ebfmi) e = cudaMemcpyAsync(ebfmi, d_f + 1, sizeof(double) * B, cudaMemcpyDeviceToHost, h->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
-  cudaFree(d_cnt); cudaFree(d_f);
-  if (e != cudaSuccess) { h->err = cudaGetErrorString(e); return DHMC_ECUDA; }
+  CK(cudaMemcpyAsync(cnt, d_cnt.get(), sizeof cnt, cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaMemcpyAsync(&acc, d_f.get(), sizeof acc, cudaMemcpyDeviceToHost, h->stream));
+  if (ebfmi) CK(cudaMemcpyAsync(ebfmi, d_f.get() + 1, sizeof(double) * B, cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
   if (depth_counts) for (int i = 0; i < 33; ++i) depth_counts[i] = (int64_t)cnt[i];
   if (termination_counts) for (int i = 0; i < 3; ++i) termination_counts[i] = (int64_t)cnt[33 + i];
   if (steps_sum) *steps_sum = (int64_t)cnt[36];
@@ -1862,18 +1866,16 @@ static int ess_rhat_groups(dhmc_handle* h, const double* draws_dev, int32_t N, i
   if (L > n - 2) L = n - 2;
   if (L < 1) L = 1;
   const size_t PD = (size_t)P * D;
-  double *d_pilot = nullptr, *d_acc = nullptr;
-  CK(cudaMalloc(&d_pilot, sizeof(double) * PD));
-  CK(cudaMalloc(&d_acc, sizeof(double) * PD * (L + 3)));
-  CK(cudaMemsetAsync(d_acc, 0, sizeof(double) * PD * (L + 3), h->stream));
-  k_pilot_mean<<<(unsigned)((PD + 127) / 128), 128, 0, h->stream>>>(draws_dev, n, N, D, B, K, off, P, d_pilot);
-  k_ess_rhat<<<h->sm_count * 8, 256, 0, h->stream>>>(draws_dev, N, n, D, B, K, off, L, d_pilot, d_acc);
+  DeviceArray<double> d_pilot, d_acc;
+  CK(d_pilot.alloc(PD));
+  CK(d_acc.alloc(PD * (L + 3)));
+  CK(cudaMemsetAsync(d_acc.get(), 0, sizeof(double) * PD * (L + 3), h->stream));
+  k_pilot_mean<<<(unsigned)((PD + 127) / 128), 128, 0, h->stream>>>(draws_dev, n, N, D, B, K, off, P, d_pilot.get());
+  k_ess_rhat<<<h->sm_count * 8, 256, 0, h->stream>>>(draws_dev, N, n, D, B, K, off, L, d_pilot.get(), d_acc.get());
   h->launches += 2;
   std::vector<double> acc(PD * (L + 3));
-  cudaError_t e = cudaMemcpyAsync(acc.data(), d_acc, sizeof(double) * acc.size(), cudaMemcpyDeviceToHost, h->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
-  cudaFree(d_pilot); cudaFree(d_acc);
-  if (e != cudaSuccess) { h->err = cudaGetErrorString(e); return DHMC_ECUDA; }
+  CK(cudaMemcpyAsync(acc.data(), d_acc.get(), sizeof(double) * acc.size(), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
   const double dn = (double)n;
   for (int g = 0; g < P; ++g) {
     // local chains of group g: [g·K, (g+1)·K) ∩ [off, off + B)
@@ -1922,17 +1924,15 @@ int dhmc_acceptance_quantiles_dev(dhmc_handle* h, const dhmc_tree_stats* stats_d
   if (!h || !stats_dev || N < 1 || !probs || nprobs < 1 || !out) return DHMC_EARG;
   CK(cudaSetDevice(h->cfg.device));
   constexpr int BINS = 4096;
-  unsigned long long* d_hist = nullptr;
-  CK(cudaMalloc(&d_hist, sizeof(unsigned long long) * (BINS + 1)));
-  CK(cudaMemsetAsync(d_hist, 0, sizeof(unsigned long long) * (BINS + 1), h->stream));
+  DeviceArray<unsigned long long> d_hist;
+  CK(d_hist.alloc(BINS + 1));
+  CK(cudaMemsetAsync(d_hist.get(), 0, sizeof(unsigned long long) * (BINS + 1), h->stream));
   const size_t n = (size_t)N * (size_t)h->cfg.n_chains;
-  k_acceptance_hist<<<h->sm_count * 8, 256, 0, h->stream>>>(stats_dev, n, d_hist, BINS);
+  k_acceptance_hist<<<h->sm_count * 8, 256, 0, h->stream>>>(stats_dev, n, d_hist.get(), BINS);
   h->launches += 1;
   std::vector<unsigned long long> hist(BINS + 1);
-  cudaError_t e = cudaMemcpyAsync(hist.data(), d_hist, sizeof(unsigned long long) * hist.size(), cudaMemcpyDeviceToHost, h->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
-  cudaFree(d_hist);
-  if (e != cudaSuccess) { h->err = cudaGetErrorString(e); return DHMC_ECUDA; }
+  CK(cudaMemcpyAsync(hist.data(), d_hist.get(), sizeof(unsigned long long) * hist.size(), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
   // the non-NaN rates in bins 1 … BINS of the grid (0, 1, BINS), both tails empty: every order statistic is placed
   // strictly inside its bin, so less than one bin width from the true value
   std::vector<unsigned long long> cum(BINS + 2, 0);
@@ -1957,10 +1957,10 @@ int dhmc_phase_clocks(dhmc_handle* h, uint64_t* out, int reset) {
   const size_t n = (size_t)kPhCount * 32 * (size_t)h->sm_count;
   std::vector<unsigned long long> v(n);
   CK(cudaDeviceSynchronize());
-  CK(cudaMemcpy(v.data(), h->phase_clocks, sizeof(unsigned long long) * n, cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(v.data(), h->phase_clocks.get(), sizeof(unsigned long long) * n, cudaMemcpyDeviceToHost));
   for (int k = 0; k < kPhCount; ++k) out[k] = 0;
   for (size_t i = 0; i < n; ++i) out[i % kPhCount] += v[i];
-  if (reset) CK(cudaMemset(h->phase_clocks, 0, sizeof(unsigned long long) * n));
+  if (reset) CK(cudaMemset(h->phase_clocks.get(), 0, sizeof(unsigned long long) * n));
   return DHMC_OK;
 }
 #endif
@@ -2045,7 +2045,7 @@ int dhmc_allgather_dev(dhmc_handle* h, const double* send_dev, double* recv_dev,
 // The current position of every chain of every rank: recv_dev [D, B·nranks] (DEVICE), one all-gather of D·B doubles per rank.
 int dhmc_allgather_positions_dev(dhmc_handle* h, double* recv_dev) {
   if (!h || !recv_dev) return DHMC_EARG;
-  return dhmc_allgather_dev(h, h->q, recv_dev, (size_t)h->cfg.n_chains * (size_t)h->cfg.dim);
+  return dhmc_allgather_dev(h, h->q.get(), recv_dev, (size_t)h->cfg.n_chains * (size_t)h->cfg.dim);
 }
 int dhmc_last_comm_ms(dhmc_handle* h, double* ms) { if (!h || !ms) return DHMC_EARG; *ms = h->last_comm_ms; return DHMC_OK; }
 #undef CKN
