@@ -1133,11 +1133,6 @@ int dhmc_find_initial_stepsize(dhmc_handle* h, double initial_eps, double log_th
   return rc;
 }
 
-// common driver of sample_tree / warmup stage / mcmc.
-// Host outputs of large runs are pipelined: the chains are cut into chunks, each
-// chunk is one k_nuts launch on the compute stream, and its draws/statistics are
-// copied D2H on the copy stream while the next chunk computes (pinned host
-// buffers make the copies truly asynchronous; pageable ones still work).
 // Is `p` page-locked host memory that the device can address (cudaHostAlloc / cudaHostRegister)?  Then *dev is its device alias.
 static bool host_mapped(const void* p, void** dev) {
   const char* evn = std::getenv("DHMC_NO_DIRECT");        // A/B switch: always stage
@@ -1148,18 +1143,33 @@ static bool host_mapped(const void* p, void** dev) {
   *dev = at.devicePointer;
   return true;
 }
-static int run_nuts(dhmc_handle* h, int N, const AdaptConfig& cfg, double lambda, const double* p_over_host,
-                    const uint32_t* dir_over_host, double* posterior, dhmc_tree_stats* stats,
-                    double* eps_used, double* logdens, bool outputs_on_device, bool advance_t,
-                    const double* q_host = nullptr, int thin = 1, bool pool_metric = false,
-                    const SummaryArgs* summary = nullptr) {
-  if ((!h->has_position && !q_host) || !h->has_eps) { h->err = "set position and step size (or run the initial search) first"; return DHMC_EARG; }
+
+// One call of run_nuts: N transitions per chain, every thin-th one kept.  A caller sets the fields it uses.
+struct NutsRequest {
+  int N = 0, thin = 1;
+  AdaptConfig cfg{};                            // warm-up: step-size adaptation and the metric to estimate
+  double lambda = 0.0;                          // warm-up: regularisation λ of an estimated Symmetric metric
+  bool pool_metric = false;                     // warm-up: pool that estimate over groups of 8 chains
+  const double* q_host = nullptr;               // host positions [B][D] to start from (NULL: the handle's)
+  const double* p_over_host = nullptr; const uint32_t* dir_over_host = nullptr;   // dhmc_sample_tree: momenta, directions
+  // outputs in the order of h->stage: draws, tree statistics, step sizes, log densities (NULL: not kept)
+  double* posterior = nullptr; dhmc_tree_stats* stats = nullptr; double* eps_used = nullptr; double* logdens = nullptr;
+  bool outputs_on_device = false;               // the outputs are device arrays
+  const SummaryArgs* summary = nullptr;         // device SummaryArgs: fold the kept draws into the streaming summary
+};
+
+// Common driver of sample_tree / warmup stage / mcmc / mcmc_summary; the transition count advances by N.  Host outputs of
+// large runs are pipelined: the chains are cut into chunks, each chunk is one k_nuts launch on the compute stream, and its
+// draws/statistics are copied D2H on the copy stream while the next chunk computes (pinned host buffers make the copies
+// truly asynchronous; pageable ones still work).
+static int run_nuts(dhmc_handle* h, const NutsRequest& r) {
+  if ((!h->has_position && !r.q_host) || !h->has_eps) { h->err = "set position and step size (or run the initial search) first"; return DHMC_EARG; }
   const auto tr0 = std::chrono::steady_clock::now();
   auto tr_ms = [&] { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - tr0).count(); };
   double tr_pt[6] = {0, 0, 0, 0, 0, 0};
   CK(cudaSetDevice(h->cfg.device));
-  if (thin < 1 || N % thin != 0) { h->err = "thin >= 1 and N a multiple of thin"; return DHMC_EARG; }
-  const size_t B = (size_t)h->cfg.n_chains, D = (size_t)h->cfg.dim, n = (size_t)(N / thin);   // n: kept draws per chain
+  if (r.thin < 1 || r.N % r.thin != 0) { h->err = "thin >= 1 and N a multiple of thin"; return DHMC_EARG; }
+  const size_t B = (size_t)h->cfg.n_chains, D = (size_t)h->cfg.dim, n = (size_t)(r.N / r.thin);   // n: kept draws per chain
   double* d_p = nullptr;
   unsigned* d_dir = nullptr;
   int rc = DHMC_OK;
@@ -1168,12 +1178,12 @@ static int run_nuts(dhmc_handle* h, int N, const AdaptConfig& cfg, double lambda
   // device memory.  Pageable buffers are staged in HBM (out[i] in stage[i]) and copied chunk by chunk; if the draws would
   // not fit, the buffer is page-locked on the fly (cudaHostRegister) and written directly.
   struct Output { void* host; size_t row; void* dev; bool direct; };       // row: bytes per kept draw of a chain
-  Output out[4] = {{posterior, sizeof(double) * D, nullptr, false}, {stats, sizeof(dhmc_tree_stats), nullptr, false},
-                   {eps_used, sizeof(double), nullptr, false}, {logdens, sizeof(double), nullptr, false}};
+  Output out[4] = {{r.posterior, sizeof(double) * D, nullptr, false}, {r.stats, sizeof(dhmc_tree_stats), nullptr, false},
+                   {r.eps_used, sizeof(double), nullptr, false}, {r.logdens, sizeof(double), nullptr, false}};
   for (int i = 0; i < 4; ++i) {
     Output& o = out[i];
     if (!o.host) continue;
-    if (outputs_on_device) { o.dev = o.host; continue; }
+    if (r.outputs_on_device) { o.dev = o.host; continue; }
     const size_t bytes = o.row * B * n;
     if (i == 0) {
       // Draws: staging + DMA copies overlapped chunk by chunk is the faster route when the draws fit in HBM (C2: 21.9 ms per
@@ -1203,32 +1213,32 @@ static int run_nuts(dhmc_handle* h, int N, const AdaptConfig& cfg, double lambda
       o.dev = h->stage[i].get();
     }
   }
-  if (p_over_host) {
+  if (r.p_over_host) {
     CK(h->tmp_bd.grow(B * D));
     d_p = h->tmp_bd.get();
-    CK(cudaMemcpyAsync(d_p, p_over_host, sizeof(double) * B * D, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(d_p, r.p_over_host, sizeof(double) * B * D, cudaMemcpyHostToDevice, h->stream));
   }
-  if (dir_over_host) {
+  if (r.dir_over_host) {
     CK(h->tmp_dir.grow(B));
     d_dir = h->tmp_dir.get();
-    CK(cudaMemcpyAsync(d_dir, dir_over_host, sizeof(unsigned) * B, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(d_dir, r.dir_over_host, sizeof(unsigned) * B, cudaMemcpyHostToDevice, h->stream));
   }
   tr_pt[0] = tr_ms();
   KArgs a = base_args(h);
-  a.N = N; a.thin = thin; a.N_keep = (int)n; a.cfg = cfg; a.p_override = d_p; a.dir_override = d_dir;
+  a.N = r.N; a.thin = r.thin; a.N_keep = (int)n; a.cfg = r.cfg; a.p_override = d_p; a.dir_override = d_dir;
   a.out_q = (double*)out[0].dev; a.out_stats = (dhmc_tree_stats*)out[1].dev; a.out_eps = (double*)out[2].dev;
   a.out_lq = (double*)out[3].dev;
-  if (cfg.metric == DHMC_METRIC_SYMMETRIC) a.covt = h->covt.get();
-  if (pool_metric) a.mean_out = h->mean_pool.get();
-  a.summary = summary;
-  const size_t out_bytes = posterior ? sizeof(double) * B * n * D : 0;
+  if (r.cfg.metric == DHMC_METRIC_SYMMETRIC) a.covt = h->covt.get();
+  if (r.pool_metric) a.mean_out = h->mean_pool.get();
+  a.summary = r.summary;
+  const size_t out_bytes = r.posterior ? sizeof(double) * B * n * D : 0;
   // chunks must stay many waves long, or the ragged tail of every chunk idles the SMs
   // chunks overlap the staged downloads (and the upload of q_host) with the sampling of the next chunk; with direct
   // host writes only an upload is left to overlap
-  const bool staged_big = posterior && !out[0].direct && out_bytes >= ((size_t)32 << 20);
-  int nchunks = (!outputs_on_device && B >= 4096 && (staged_big || q_host)) ? 16 : 1;
+  const bool staged_big = r.posterior && !out[0].direct && out_bytes >= ((size_t)32 << 20);
+  int nchunks = (!r.outputs_on_device && B >= 4096 && (staged_big || r.q_host)) ? 16 : 1;
   while (nchunks > 1 && B / (size_t)nchunks < (size_t)8 * (size_t)h->grid * (size_t)h->G) nchunks /= 2;   // >= 8 waves of chain slots per chunk
-  if (const char* ev = std::getenv("DHMC_E2E_CHUNKS")) { const int v = std::atoi(ev); if (v >= 1 && v <= 16 && !outputs_on_device) nchunks = v; }
+  if (const char* ev = std::getenv("DHMC_E2E_CHUNKS")) { const int v = std::atoi(ev); if (v >= 1 && v <= 16 && !r.outputs_on_device) nchunks = v; }
   CK(cudaMemsetAsync(h->status.get(), 0, sizeof(int) * B, h->stream));   // status words describe the current call
   for (int ci = 0; ci < nchunks; ++ci) {
     // (a pooled metric, and a batch on packed groups, keep their groups of 8 chains inside one chunk)
@@ -1236,14 +1246,14 @@ static int run_nuts(dhmc_handle* h, int N, const AdaptConfig& cfg, double lambda
     const size_t c0 = (B / unit) * ci / nchunks * unit, c1 = (B / unit) * (ci + 1) / nchunks * unit, nc = c1 - c0;
     if (nc == 0) continue;
     a.chain_begin = (int)c0; a.chain_end = (int)c1;
-    if (q_host) {
+    if (r.q_host) {
       // positions of this chunk: H2D on its own stream, then evaluate_ℓ(strict) on the compute
       // stream — overlaps with the previous chunk's sampling and D2H
       if (ci == 0) {   // uploads start after everything already queued on the compute stream
         CK(cudaEventRecord(h->h2d_ev[15], h->stream));
         CK(cudaStreamWaitEvent(h->h2d_stream, h->h2d_ev[15], 0));
       }
-      CK(cudaMemcpyAsync(h->q.get() + c0 * D, q_host + c0 * D, sizeof(double) * nc * D, cudaMemcpyHostToDevice, h->h2d_stream));
+      CK(cudaMemcpyAsync(h->q.get() + c0 * D, r.q_host + c0 * D, sizeof(double) * nc * D, cudaMemcpyHostToDevice, h->h2d_stream));
       CK(cudaEventRecord(h->h2d_ev[ci], h->h2d_stream));
       CK(cudaStreamWaitEvent(h->stream, h->h2d_ev[ci], 0));
       KArgs ea = a;
@@ -1254,7 +1264,7 @@ static int run_nuts(dhmc_handle* h, int N, const AdaptConfig& cfg, double lambda
     // the kernel time of the call: from the first chunk's k_nuts to the end of the last one's
     rc = launch(h, K_NUTS, a, ci == 0 ? h->ev0 : nullptr, ci == nchunks - 1 ? h->ev1 : nullptr, ci == 0);
     if (rc != DHMC_OK) return rc;
-    if (!outputs_on_device) {
+    if (!r.outputs_on_device) {
       CK(cudaEventRecord(h->chunk_ev[ci], h->stream));
       CK(cudaStreamWaitEvent(h->copy_stream, h->chunk_ev[ci], 0));
       for (const Output& o : out)
@@ -1278,9 +1288,9 @@ static int run_nuts(dhmc_handle* h, int N, const AdaptConfig& cfg, double lambda
     std::fprintf(stderr, "[dhmc trace] chunks %d:", nchunks);
     for (int ci = 0; ci < nchunks; ++ci) {
       float a = -1, b2 = -1, c = -1;
-      if (q_host) cudaEventElapsedTime(&a, h->ev0, h->h2d_ev[ci]);
+      if (r.q_host) cudaEventElapsedTime(&a, h->ev0, h->h2d_ev[ci]);
       cudaEventElapsedTime(&b2, h->ev0, h->chunk_ev[ci]);
-      if (!outputs_on_device) cudaEventElapsedTime(&c, h->ev0, h->copy_ev[ci]);
+      if (!r.outputs_on_device) cudaEventElapsedTime(&c, h->ev0, h->copy_ev[ci]);
       std::fprintf(stderr, " [h2d %.2f kern %.2f d2h %.2f]", a, b2, c);
     }
     cudaEventElapsedTime(&t, h->ev0, h->ev1);
@@ -1289,33 +1299,33 @@ static int run_nuts(dhmc_handle* h, int N, const AdaptConfig& cfg, double lambda
     cudaGetLastError();
   }
   h->last_steps = (int64_t)steps;
-  if (advance_t) h->t += (uint32_t)N;
-  if (q_host) h->has_position = true;
+  h->t += (uint32_t)r.N;
+  if (r.q_host) h->has_position = true;
   if (h->trace) std::fprintf(stderr, "[dhmc trace] host: before status check %.2f ms\n", tr_ms());
   rc = sync_and_check_status(h, DHMC_CHAIN_NONFINITE_Q | DHMC_CHAIN_BAD_ACCEPTANCE | DHMC_CHAIN_BAD_STEPSIZE |
-                                    DHMC_CHAIN_LEAPFROG_NONFINITE | (q_host ? DHMC_CHAIN_BAD_INITIAL : 0),
-                             q_host ? "invalid initial position, or non-finite position / acceptance rate / step size while sampling"
+                                    DHMC_CHAIN_LEAPFROG_NONFINITE | (r.q_host ? DHMC_CHAIN_BAD_INITIAL : 0),
+                             r.q_host ? "invalid initial position, or non-finite position / acceptance rate / step size while sampling"
                                     : "sampling: non-finite position, acceptance rate or step size");
   if (h->trace) std::fprintf(stderr, "[dhmc trace] host: after status check %.2f ms\n", tr_ms());
   if (rc != DHMC_OK) return rc;
-  if (cfg.metric == DHMC_METRIC_DIAGONAL) return set_metric_kind(h, false, false);   // κ ← Diagonal: the diagonal kernels
-  if (cfg.metric == DHMC_METRIC_SYMMETRIC) {
+  if (r.cfg.metric == DHMC_METRIC_DIAGONAL) return set_metric_kind(h, false, false);   // κ ← Diagonal: the diagonal kernels
+  if (r.cfg.metric == DHMC_METRIC_SYMMETRIC) {
     // κ = GaussianKineticEnergy(regularize_M⁻¹(sample_M⁻¹(Symmetric, X), λ)) — mcmc.jl:282
     const int fgrid = factor_grid(h);
-    if (pool_metric)
-      k_cov_pool<<<fgrid, 128, sizeof(double) * h->cfg.dim, h->stream>>>(h->covt.get(), h->mean_pool.get(), h->minv_dense.get(), N, lambda, (int)h->cfg.dim, (int)h->cfg.n_chains);
+    if (r.pool_metric)
+      k_cov_pool<<<fgrid, 128, sizeof(double) * h->cfg.dim, h->stream>>>(h->covt.get(), h->mean_pool.get(), h->minv_dense.get(), r.N, r.lambda, (int)h->cfg.dim, (int)h->cfg.n_chains);
     else
-      k_cov_finish<<<fgrid, 128, 0, h->stream>>>(h->covt.get(), h->minv_dense.get(), N, lambda, (int)h->cfg.dim, (int)h->cfg.n_chains);
+      k_cov_finish<<<fgrid, 128, 0, h->stream>>>(h->covt.get(), h->minv_dense.get(), r.N, r.lambda, (int)h->cfg.dim, (int)h->cfg.n_chains);
     h->launches += 1;
-    rc = factor_and_switch(h, pool_metric);
+    rc = factor_and_switch(h, r.pool_metric);
   }
   return rc;
 }
 
 int dhmc_sample_tree(dhmc_handle* h, const double* p, const uint32_t* directions, dhmc_tree_stats* stats) {
   if (!h) return DHMC_EARG;
-  AdaptConfig cfg{};
-  return run_nuts(h, 1, cfg, 0.0, p, directions, nullptr, stats, nullptr, nullptr, false, true);
+  NutsRequest r; r.N = 1; r.p_over_host = p; r.dir_over_host = directions; r.stats = stats;
+  return run_nuts(h, r);
 }
 
 int dhmc_warmup_stage(dhmc_handle* h, int32_t N, int32_t metric, const dhmc_dual_averaging* da,
@@ -1330,37 +1340,38 @@ int dhmc_warmup_stage(dhmc_handle* h, int32_t N, int32_t metric, const dhmc_dual
   const bool pool = metric == DHMC_METRIC_SYMMETRIC_POOLED;
   if (pool && (h->cfg.n_chains % 8 != 0 || h->cfg.chain_offset % 8 != 0)) { h->err = "pooled metric: n_chains and chain_offset must be multiples of 8"; return DHMC_EARG; }
   if (pool && h->batch_k % 8 != 0) { h->err = "pooled metric with a problem batch: chains_per_problem must be a multiple of 8 (a metric group never straddles two problems)"; return DHMC_EARG; }
-  AdaptConfig cfg{};
-  cfg.metric = pool ? DHMC_METRIC_SYMMETRIC : metric;
+  NutsRequest r; r.N = N; r.lambda = lambda; r.pool_metric = pool;
+  r.posterior = posterior; r.stats = stats; r.eps_used = eps_used; r.logdens = logdens;
+  r.cfg.metric = pool ? DHMC_METRIC_SYMMETRIC : metric;
   if (da) {
     // DualAveraging @argchecks — stepsize.jl:108-111
     if (!(0 < da->delta && da->delta < 1) || !(da->gamma > 0) || !(0.5 < da->kappa && da->kappa <= 1) || !(da->t0 >= 0)) {
       h->err = "DualAveraging: 0 < δ < 1, γ > 0, 0.5 < κ ≤ 1, t₀ ≥ 0"; return DHMC_EARG;
     }
-    cfg.adapt = 1; cfg.delta = da->delta; cfg.gamma = da->gamma; cfg.kappa = da->kappa; cfg.t0 = da->t0;
+    r.cfg.adapt = 1; r.cfg.delta = da->delta; r.cfg.gamma = da->gamma; r.cfg.kappa = da->kappa; r.cfg.t0 = da->t0;
   }
-  if (cfg.metric == DHMC_METRIC_SYMMETRIC) { int rcd = ensure_dense(h); if (rcd != DHMC_OK) return rcd; }
+  if (r.cfg.metric == DHMC_METRIC_SYMMETRIC) { int rcd = ensure_dense(h); if (rcd != DHMC_OK) return rcd; }
   if (pool) CK(h->mean_pool.grow((size_t)h->cfg.n_chains * (size_t)h->cfg.dim));
-  return run_nuts(h, N, cfg, lambda, nullptr, nullptr, posterior, stats, eps_used, logdens, false, true, nullptr, 1, pool);
+  return run_nuts(h, r);
 }
 
 int dhmc_mcmc(dhmc_handle* h, int32_t N, double* posterior, dhmc_tree_stats* stats, double* logdens) {
   if (!h || N < 0) return DHMC_EARG;
   if (N == 0) return DHMC_OK;
-  AdaptConfig cfg{};
-  return run_nuts(h, N, cfg, 0.0, nullptr, nullptr, posterior, stats, nullptr, logdens, false, true);
+  NutsRequest r; r.N = N; r.posterior = posterior; r.stats = stats; r.logdens = logdens;
+  return run_nuts(h, r);
 }
 int dhmc_mcmc_from(dhmc_handle* h, const double* q, int32_t N, double* posterior, dhmc_tree_stats* stats,
                    double* logdens) {
   if (!h || !q || N < 1) return DHMC_EARG;
-  AdaptConfig cfg{};
-  return run_nuts(h, N, cfg, 0.0, nullptr, nullptr, posterior, stats, nullptr, logdens, false, true, q);
+  NutsRequest r; r.N = N; r.q_host = q; r.posterior = posterior; r.stats = stats; r.logdens = logdens;
+  return run_nuts(h, r);
 }
 int dhmc_mcmc_thinned(dhmc_handle* h, const double* q, int32_t N, int32_t thin, double* posterior,
                       dhmc_tree_stats* stats, double* logdens) {
   if (!h || N < 1 || thin < 1) return DHMC_EARG;
-  AdaptConfig cfg{};
-  return run_nuts(h, N, cfg, 0.0, nullptr, nullptr, posterior, stats, nullptr, logdens, false, true, q, thin);
+  NutsRequest r; r.N = N; r.thin = thin; r.q_host = q; r.posterior = posterior; r.stats = stats; r.logdens = logdens;
+  return run_nuts(h, r);
 }
 // Page-locked host memory on the NUMA node of the handle's GPU: the calling thread is moved to that node's CPUs while the
 // pages are allocated and pinned (first touch), so that the kernel's direct writes / the DMA engines cross one PCIe root
@@ -1413,14 +1424,11 @@ int dhmc_host_free(dhmc_handle* h, void* p) {
 int dhmc_mcmc_dev(dhmc_handle* h, int32_t N, double* posterior, dhmc_tree_stats* stats, double* logdens) {
   if (!h || N < 0) return DHMC_EARG;
   if (N == 0) return DHMC_OK;
-  AdaptConfig cfg{};
-  return run_nuts(h, N, cfg, 0.0, nullptr, nullptr, posterior, stats, nullptr, logdens, true, true);
+  NutsRequest r; r.N = N; r.posterior = posterior; r.stats = stats; r.logdens = logdens; r.outputs_on_device = true;
+  return run_nuts(h, r);
 }
 
 // ------------------------------------------------------------------ streaming posterior summary (DESIGN §4.4)
-// record [DHMC_SUMMARY_FIELDS, D, P] column-major: the fields of (parameter d, problem p) at (p·D + d)·F
-static double* summary_cell(double* record, int64_t D, int64_t p, int64_t d) { return record + ((size_t)p * D + d) * DHMC_SUMMARY_FIELDS; }
-
 // The grid of every (d, p) cell of a quantile histogram (include/dhmc.h): nbins in [1, 4096], lo < hi finite, hi − lo and
 // nbins / (hi − lo) finite (so that inv_w is a finite number)
 static bool valid_grid(const double* lo, const double* hi, int nbins, size_t cells) {
@@ -1435,7 +1443,6 @@ static bool valid_grid(const double* lo, const double* hi, int nbins, size_t cel
 
 // rows [r0, r0 + n) of every problem of a host array [P][R] into the device array [P][n]
 static cudaError_t upload_rows(double* dst, const double* src, size_t r0, size_t n, size_t R, size_t P, cudaStream_t s) {
-  if (n == R) return cudaMemcpyAsync(dst, src, sizeof(double) * P * R, cudaMemcpyHostToDevice, s);
   return cudaMemcpy2DAsync(dst, sizeof(double) * n, src + r0, sizeof(double) * R, sizeof(double) * n, P, cudaMemcpyHostToDevice, s);
 }
 
@@ -1557,6 +1564,15 @@ int dhmc_generated_keyed_dev(dhmc_handle* h, const double* theta, int64_t n, int
   return generated_dev(h, theta, n, first_problem, n_problems, true, chain, transition, out);
 }
 
+// One block of summary rows: rows r0 … r0 + n − 1 of the [·, R, P] host arrays, and the device arrays the kernels fold them
+// into.  width: state per row and resident chain group (3 for parameters, whose moments live in the metric slots; 5 for G).
+struct SummaryRows {
+  size_t r0, n, width;
+  double *acc = nullptr, *shift = nullptr, *ref = nullptr, *row = nullptr, *lo = nullptr, *inv_w = nullptr;
+  unsigned long long *below = nullptr, *hist = nullptr;
+  unsigned* stage = nullptr;
+};
+
 // dhmc_mcmc_summary and, with counts, dhmc_mcmc_summary_histogram (arguments checked by the caller)
 static int mcmc_summary(dhmc_handle* h, int32_t N, int32_t thin, const double* reference, const double* lo_host,
                         const double* hi_host, int32_t nbins, double* record, int64_t* counts, dhmc_tree_stats* stats,
@@ -1567,63 +1583,62 @@ static int mcmc_summary(dhmc_handle* h, int32_t N, int32_t thin, const double* r
   if (!record) { h->err = "dhmc_mcmc_summary: record is NULL"; return DHMC_EARG; }
   if (!h->has_position || !h->has_eps) { h->err = "set position and step size (or run the initial search) first"; return DHMC_EARG; }
   CK(cudaSetDevice(h->cfg.device));
-  const size_t D = (size_t)h->cfg.dim, B = (size_t)h->cfg.n_chains;
+  // generated quantities: ng rows after the D parameter rows of every host array (R = D + ng); empty with ng = 0
+  const size_t D = (size_t)h->cfg.dim, B = (size_t)h->cfg.n_chains, ng = (size_t)h->ngq, R = D + ng;
   const int64_t K = h->batch_k, off = h->cfg.chain_offset;
-  const size_t P = K ? (size_t)h->batch_p : 1, PD = P * D, rows = (size_t)h->grid * h->G * 3 * D;
-  // histograms (counts != NULL): cells bins per (d, p); the staging rows of the resident chain groups
-  const size_t cells = counts ? (size_t)nbins + 2 : 0, stage = (size_t)h->grid * h->G * cells * D;
-  // generated quantities: ng rows after the D parameter rows of every host array (R = D + ng rows), and on the device the
-  // arrays of SummaryArgs' g-fields, laid out as the parameters' with ng in place of D
-  const size_t ng = (size_t)h->ngq, R = D + ng, PG = P * ng, grows = (size_t)h->grid * h->G * 5 * ng;
-  const size_t gstage = (size_t)h->grid * h->G * cells * ng;
+  // histograms (counts != NULL): cells bins per (row, problem), and staging rows [cells][n] per resident chain group
+  const size_t P = K ? (size_t)h->batch_p : 1, groups = (size_t)h->grid * h->G, cells = counts ? (size_t)nbins + 2 : 0;
+  SummaryRows blk[2] = {{0, D, 3}, {D, ng, 5}};
+  SummaryRows &par = blk[0], &gen = blk[1];
+  unsigned long long* chains;                  // completed chains per problem [P]
+  int64_t* kchain = nullptr;                   // keys of the generated shift's points, chain [P] and transition [P]
+  uint32_t* ktrans = nullptr;
   // one grow-only arena of the arrays below, in this order (8-byte elements, then the 4-byte staging rows, then the 8-aligned
   // keys of random generated quantities): carve(nullptr) measures it, carve(base) places the arrays in it
-  double *acc, *shift, *ref, *row, *lo = nullptr, *inv_w = nullptr, *gacc, *gshift, *gref, *grow, *glo = nullptr, *ginv_w = nullptr;
-  unsigned long long *below, *chains, *hist, *gbelow, *ghist;
-  unsigned *stg, *gstg;                        // histogram staging rows [grid·G][cells][D], [grid·G][cells][ng]
-  int64_t* kchain = nullptr;                   // keys of the shift's points, chain [P] and transition [P]
-  uint32_t* ktrans = nullptr;
   auto carve = [&](char* base) {
     size_t at = 0;
     auto take = [&](auto& ptr, size_t n) {
       ptr = base ? reinterpret_cast<std::remove_reference_t<decltype(ptr)>>(base + at) : nullptr;
       at += sizeof(*ptr) * n;
     };
-    take(acc, 5 * PD); take(shift, PD); take(ref, PD); take(row, rows); take(below, PD); take(chains, P); take(hist, PD * cells);
-    if (counts) { take(lo, PD); take(inv_w, PD); }
-    take(gacc, 5 * PG); take(gshift, PG); take(gref, PG); take(grow, grows); take(gbelow, PG); take(ghist, PG * cells);
-    if (counts) { take(glo, PG); take(ginv_w, PG); }
-    take(stg, stage); take(gstg, gstage);
+    for (SummaryRows& b : blk) {             // acc, below and hist adjacent: one memset zeroes them
+      const size_t pn = P * b.n;
+      take(b.acc, 5 * pn); take(b.below, pn); take(b.hist, pn * cells);
+      take(b.shift, pn); take(b.ref, pn); take(b.row, groups * b.width * b.n);
+      if (counts) { take(b.lo, pn); take(b.inv_w, pn); }
+    }
+    take(chains, P);
+    for (SummaryRows& b : blk) take(b.stage, groups * cells * b.n);
     if (h->gq_random) { at = (at + 7) & ~(size_t)7; take(kchain, P); take(ktrans, P); }
     return at;
   };
   CK(h->sum_buf.grow(carve(nullptr)));
   carve(h->sum_buf.get());
   CK(h->sum_args.grow(1));
-  CK(cudaMemsetAsync(acc, 0, sizeof(double) * 5 * PD, h->stream));
-  CK(cudaMemsetAsync(below, 0, sizeof(unsigned long long) * (PD + P), h->stream));
-  if (reference) CK(upload_rows(ref, reference, 0, D, R, P, h->stream));
+  std::vector<double> hinv(counts ? P * R : 0);
+  for (size_t i = 0; i < hinv.size(); ++i) hinv[i] = (double)nbins / (hi_host[i] - lo_host[i]);
+  for (const SummaryRows& b : blk) {
+    if (!b.n) continue;
+    CK(cudaMemsetAsync(b.acc, 0, sizeof(double) * P * b.n * (6 + cells), h->stream));
+    if (reference) CK(upload_rows(b.ref, reference, b.r0, b.n, R, P, h->stream));
+    if (counts) {
+      CK(upload_rows(b.lo, lo_host, b.r0, b.n, R, P, h->stream));
+      CK(upload_rows(b.inv_w, hinv.data(), b.r0, b.n, R, P, h->stream));
+    }
+  }
+  CK(cudaMemsetAsync(chains, 0, sizeof(unsigned long long) * P, h->stream));
   // shift of problem p: the position of its first local chain, max(p·K − off, 0); problems p0 … p1 have local chains.  Past
   // the first, those chains are K apart: one strided copy (a first problem entered in its middle takes one more).
   const int64_t p0 = K ? off / K : 0, p1 = K ? (off + (int64_t)B - 1) / K : 0;
   const int64_t pa = (K && off % K) ? p0 + 1 : p0;
-  if (pa > p0) CK(cudaMemcpyAsync(shift + p0 * D, h->q.get(), sizeof(double) * D, cudaMemcpyDeviceToDevice, h->stream));
+  if (pa > p0) CK(cudaMemcpyAsync(par.shift + p0 * D, h->q.get(), sizeof(double) * D, cudaMemcpyDeviceToDevice, h->stream));
   if (p1 >= pa)
-    CK(cudaMemcpy2DAsync(shift + pa * D, sizeof(double) * D, h->q.get() + (size_t)(K ? pa * K - off : 0) * D, sizeof(double) * D * (size_t)(K ? K : 1),
+    CK(cudaMemcpy2DAsync(par.shift + pa * D, sizeof(double) * D, h->q.get() + (size_t)(K ? pa * K - off : 0) * D, sizeof(double) * D * (size_t)(K ? K : 1),
                          sizeof(double) * D, (size_t)(p1 - pa + 1), cudaMemcpyDeviceToDevice, h->stream));
-  SummaryArgs sa{row, shift, reference ? ref : nullptr, acc, below, chains, n_keep / 2, nullptr, nullptr, nullptr, nullptr, 0};
-  std::vector<double> hinv(counts ? P * R : 0);
-  for (size_t i = 0; i < hinv.size(); ++i) hinv[i] = (double)nbins / (hi_host[i] - lo_host[i]);
-  if (counts) {
-    CK(cudaMemsetAsync(hist, 0, sizeof(unsigned long long) * PD * cells, h->stream));
-    CK(upload_rows(lo, lo_host, 0, D, R, P, h->stream));
-    CK(upload_rows(inv_w, hinv.data(), 0, D, R, P, h->stream));
-    sa.lo = lo; sa.inv_w = inv_w; sa.stage = stg; sa.hist = hist; sa.nbins = nbins;
-  }
+  SummaryArgs sa{par.row, par.shift, reference ? par.ref : nullptr, par.acc, par.below, chains, n_keep / 2, nullptr, nullptr, nullptr, nullptr, 0};
+  if (counts) { sa.lo = par.lo; sa.inv_w = par.inv_w; sa.stage = par.stage; sa.hist = par.hist; sa.nbins = nbins; }
   // generated quantities: the shift is g(shift), evaluated on the device
   if (ng) {
-    CK(cudaMemsetAsync(gacc, 0, sizeof(double) * 5 * PG, h->stream));
-    CK(cudaMemsetAsync(gbelow, 0, sizeof(unsigned long long) * PG, h->stream));
     // random quantities: the shift's key is (global id of the problem's first local chain, the call's first transition);
     // it only sets the cancellation shift of the sums
     if (h->gq_random) {
@@ -1634,63 +1649,47 @@ static int mcmc_summary(dhmc_handle* h, int32_t N, int32_t thin, const double* r
       CK(cudaMemcpyAsync(kchain, hc.data(), sizeof(int64_t) * np, cudaMemcpyHostToDevice, h->stream));
       CK(cudaMemcpyAsync(ktrans, ht.data(), sizeof(uint32_t) * np, cudaMemcpyHostToDevice, h->stream));
     }
-    const int rg = launch_generated(h, shift + p0 * D, 1, p0, p1 - p0 + 1, kchain, ktrans, gshift + p0 * ng);
+    const int rg = launch_generated(h, par.shift + p0 * D, 1, p0, p1 - p0 + 1, kchain, ktrans, gen.shift + p0 * ng);
     if (rg != DHMC_OK) return rg;
-    if (reference) CK(upload_rows(gref, reference, D, ng, R, P, h->stream));
     sa.ng = (int)ng; sa.mparams = h->mparams.get(); sa.problems = K ? h->problems.get() : nullptr;
     sa.seed = (unsigned long long)h->cfg.seed; sa.chain_offset = (long long)off; sa.t0 = h->t; sa.thin = thin;
-    sa.grow = grow; sa.gshift = gshift; sa.gref = reference ? gref : nullptr; sa.gacc = gacc; sa.gbelow = gbelow;
-    if (counts) {
-      CK(cudaMemsetAsync(ghist, 0, sizeof(unsigned long long) * PG * cells, h->stream));
-      CK(upload_rows(glo, lo_host, D, ng, R, P, h->stream));
-      CK(upload_rows(ginv_w, hinv.data(), D, ng, R, P, h->stream));
-      sa.glo = glo; sa.ginv_w = ginv_w; sa.gstage = gstg; sa.ghist = ghist;
-    }
+    sa.grow = gen.row; sa.gshift = gen.shift; sa.gref = reference ? gen.ref : nullptr; sa.gacc = gen.acc; sa.gbelow = gen.below;
+    if (counts) { sa.glo = gen.lo; sa.ginv_w = gen.inv_w; sa.gstage = gen.stage; sa.ghist = gen.hist; }
   }
   CK(cudaMemcpyAsync(h->sum_args.get(), &sa, sizeof sa, cudaMemcpyHostToDevice, h->stream));
-  AdaptConfig cfg{};
-  const int rc = run_nuts(h, N, cfg, 0.0, nullptr, nullptr, nullptr, stats, nullptr, logdens, false, true, nullptr, thin, false,
-                          h->sum_args.get());
+  NutsRequest req; req.N = N; req.thin = thin; req.stats = stats; req.logdens = logdens; req.summary = h->sum_args.get();
+  const int rc = run_nuts(h, req);
   if (rc != DHMC_OK && rc != DHMC_ENUMERIC) return rc;    // a chain that failed is left out of its problem's sums
-  std::vector<double> hacc(5 * PD), hshift(PD), hgacc(5 * PG), hgshift(PG);
-  std::vector<unsigned long long> hcnt(PD + P), hgcnt(PG);
-  CK(cudaMemcpyAsync(hacc.data(), acc, sizeof(double) * hacc.size(), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaMemcpyAsync(hshift.data(), shift, sizeof(double) * PD, cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaMemcpyAsync(hcnt.data(), below, sizeof(unsigned long long) * hcnt.size(), cudaMemcpyDeviceToHost, h->stream));
-  // [P][D][cells] is the column-major [cells, D, P] of the ABI; uint64 counts stay far below 2^63
-  if (counts && !ng) CK(cudaMemcpyAsync(counts, hist, sizeof(int64_t) * PD * cells, cudaMemcpyDeviceToHost, h->stream));
-  if (ng) {            // counts [cells, R, P]: the D parameter rows, then the ng generated rows of each problem
-    CK(cudaMemcpyAsync(hgacc.data(), gacc, sizeof(double) * hgacc.size(), cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaMemcpyAsync(hgshift.data(), gshift, sizeof(double) * PG, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaMemcpyAsync(hgcnt.data(), gbelow, sizeof(unsigned long long) * PG, cudaMemcpyDeviceToHost, h->stream));
-    if (counts) {
-      const size_t c8 = sizeof(int64_t) * cells;
-      CK(cudaMemcpy2DAsync(counts, c8 * R, hist, c8 * D, c8 * D, P, cudaMemcpyDeviceToHost, h->stream));
-      CK(cudaMemcpy2DAsync(counts + D * cells, c8 * R, ghist, c8 * ng, c8 * ng, P, cudaMemcpyDeviceToHost, h->stream));
-    }
+  // host copies: a block's sums [P][5][n], shifts and below-counts [P][n] at P·r0
+  std::vector<double> hacc(5 * P * R), hshift(P * R);
+  std::vector<unsigned long long> hbelow(P * R), hchains(P);
+  for (const SummaryRows& b : blk) {
+    if (!b.n) continue;
+    const size_t at = P * b.r0, pn = P * b.n, c8 = sizeof(int64_t) * cells;
+    CK(cudaMemcpyAsync(&hacc[5 * at], b.acc, sizeof(double) * 5 * pn, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(&hshift[at], b.shift, sizeof(double) * pn, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(&hbelow[at], b.below, sizeof(unsigned long long) * pn, cudaMemcpyDeviceToHost, h->stream));
+    // [P][n][cells] into rows r0 … r0 + n − 1 of the column-major [cells, R, P] of the ABI; uint64 counts stay far below 2^63
+    if (counts) CK(cudaMemcpy2DAsync(counts + b.r0 * cells, c8 * R, b.hist, c8 * b.n, c8 * b.n, P, cudaMemcpyDeviceToHost, h->stream));
   }
+  CK(cudaMemcpyAsync(hchains.data(), chains, sizeof(unsigned long long) * P, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
-  // row d of problem p from its sums a[·], its shift and its below-count (the sums of n rows, [5][n])
-  auto finish = [&](size_t p, size_t r_out, const double* a, size_t n, size_t d, double sh, unsigned long long nb) {
-    const double M = (double)hcnt[PD + p], m = 2.0 * M;
-    double* r = summary_cell(record, (int64_t)R, (int64_t)p, (int64_t)r_out);
-    r[DHMC_SUMMARY_CHAINS] = M;
-    r[DHMC_SUMMARY_NKEEP] = (double)n_keep;
-    r[DHMC_SUMMARY_BELOW] = reference ? (double)nb : dm_nan();
-    if (M == 0) {
-      r[DHMC_SUMMARY_MEAN] = r[DHMC_SUMMARY_SS_SEQ] = r[DHMC_SUMMARY_M2] = r[DHMC_SUMMARY_SS_CHAIN] = 0.0;
-      return;
-    }
-    const double s1 = a[d], s2 = a[n + d], c1 = a[3 * n + d], c2 = a[4 * n + d];
-    r[DHMC_SUMMARY_MEAN] = sh + s1 / m;
-    r[DHMC_SUMMARY_SS_SEQ] = std::max(0.0, s2 - s1 * s1 / m);
-    r[DHMC_SUMMARY_M2] = a[2 * n + d];
-    r[DHMC_SUMMARY_SS_CHAIN] = std::max(0.0, c2 - c1 * c1 / M);
-  };
-  for (size_t p = 0; p < P; ++p) {
-    for (size_t d = 0; d < D; ++d) finish(p, d, &hacc[p * 5 * D], D, d, hshift[p * D + d], hcnt[p * D + d]);
-    for (size_t k = 0; k < ng; ++k) finish(p, D + k, &hgacc[p * 5 * ng], ng, k, hgshift[p * ng + k], hgcnt[p * ng + k]);
-  }
+  // record [F, R, P] column-major: the cell of row r0 + k of problem p, from its sums a ([5][n]), shift and below-count
+  for (size_t p = 0; p < P; ++p)
+    for (const SummaryRows& b : blk)
+      for (size_t k = 0, i = P * b.r0 + p * b.n; k < b.n; ++k) {
+        const double M = (double)hchains[p], m = 2.0 * M, *a = &hacc[5 * i];
+        double* r = record + (p * R + b.r0 + k) * DHMC_SUMMARY_FIELDS;
+        r[DHMC_SUMMARY_CHAINS] = M;
+        r[DHMC_SUMMARY_NKEEP] = (double)n_keep;
+        r[DHMC_SUMMARY_BELOW] = reference ? (double)hbelow[i + k] : dm_nan();
+        if (M == 0) { r[DHMC_SUMMARY_MEAN] = r[DHMC_SUMMARY_SS_SEQ] = r[DHMC_SUMMARY_M2] = r[DHMC_SUMMARY_SS_CHAIN] = 0.0; continue; }
+        const double s1 = a[k], s2 = a[b.n + k], c1 = a[3 * b.n + k], c2 = a[4 * b.n + k];
+        r[DHMC_SUMMARY_MEAN] = hshift[i + k] + s1 / m;
+        r[DHMC_SUMMARY_SS_SEQ] = std::max(0.0, s2 - s1 * s1 / m);
+        r[DHMC_SUMMARY_M2] = a[2 * b.n + k];
+        r[DHMC_SUMMARY_SS_CHAIN] = std::max(0.0, c2 - c1 * c1 / M);
+      }
   return rc;
 }
 
